@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """bench.py — rows/sec of the hot path on synthetic TPC-DS-shaped batches (BASELINE.json metric:
-"rows/sec on TPC-DS q1 hash-agg+filter at 1/2/4/8 B200; HBM GB/s vs 8 TB/s").
+"rows/sec on TPC-DS q1 hash-agg+filter at 1/2/4/8 H100; HBM GB/s vs 3.35 TB/s").
 
 Headline workload (config.workload = "M2", SURVEY.md §8d): the q1-shaped FUSED FilterExec -> HashAggregateExec:
     Filter[f >= 200, f <= 399] (s = 0.2) -> SUM(v) GROUP BY k1, k2       f ~ U[0,1000), k1 ~ U[0,2^17), k2 ~ U[0,8),
@@ -18,7 +18,9 @@ A step = one complete aggregation of the batch: Partial -> (murmur3 pmod N excha
   verified      every timed workload's LAST result is checked after the timed region against an independent torch
                 computation (per-group sums / counts, group ownership disjoint across ranks); a mismatch exits non-zero
 
-`--impl reference` times the CPU restatement alone on the same M2 workload (the Rust reference cannot be built here).
+`--impl reference` times the CPU restatement alone on the same M2 workload.
+`--dump-outputs DIR` writes the result of the last timed M2 step as DIR/m2_<column>.npy (float64, rows sorted by group key), so that
+two builds can be compared output for output: with the same arguments the seeded inputs are identical from run to run.
 """
 import argparse
 import json
@@ -32,7 +34,8 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-METRIC = "rows/sec on TPC-DS q1 hash-agg+filter at 1/2/4/8 B200; HBM GB/s vs 8 TB/s"
+METRIC = "rows/sec on TPC-DS q1 hash-agg+filter at 1/2/4/8 H100; HBM GB/s vs 3.35 TB/s"
+HBM_PEAK_GBS = 3350.0                      # H100 SXM data sheet (HBM3, 700 W part): the roofline denominator
 CARD = 1 << 20
 K1_CARD, K2_CARD = 1 << 17, 1 << 3
 F_LO, F_HI = 200, 399
@@ -52,7 +55,7 @@ def env_int(name, default):
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
 
     def __init__(self, gpu_index):
         self.gpu = gpu_index
@@ -85,7 +88,13 @@ class ClockSampler:
         if self._t:
             self._t.join(timeout=10)
         s = sorted(self.samples)
-        return {"sm_mhz": s[len(s) // 2] if s else None, "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons), "samples": len(s)}
+        card = None                                      # a rate is only meaningful with the card and its power limit beside it
+        try:
+            card = subprocess.run(["nvidia-smi", f"--id={self.gpu}", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                                  capture_output=True, text=True, timeout=5).stdout.strip() or None
+        except Exception:
+            pass
+        return {"sm_mhz": s[len(s) // 2] if s else None, "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons), "samples": len(s), "gpu": card}
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -339,6 +348,19 @@ class Runner:
             dist.all_reduce(flag, op=dist.ReduceOp.MIN)
         return bool(flag.item()), {"groups": int(tot.item()), "sum_of_sums": int(exp_sum.sum().item())}
 
+    def dump(self, out_dir):
+        """the last step's result columns as <out_dir>/m2_<name>[_rank<r>].npy, float64 (keys < 2^17 and sums < 2^53 are exact),
+        rows sorted by group key so that the library's emit order does not matter (2^20 groups x 3 columns: 24 MB)"""
+        import numpy as np
+        torch = self.torch
+        res = [device_cols(d, torch) for d in (self.last or [])]
+        cols = [torch.cat([r[i] for r in res]) for i in range(3)] if res else [torch.zeros(0, dtype=torch.int64, device=self.dev)] * 3
+        order = torch.argsort(cols[0] * K2_CARD + cols[1])
+        os.makedirs(out_dir, exist_ok=True)
+        suffix = "" if self.world == 1 else f"_rank{self.rank}"
+        for name, c in zip(("k1", "k2", "sum_v"), cols):
+            np.save(os.path.join(out_dir, f"m2_{name}{suffix}.npy"), c[order].to(torch.float64).cpu().numpy())
+
     def close(self):
         self._drop_last()
         self.cols = None
@@ -456,25 +478,13 @@ def timed(torch, dist, world, dev, fn, steps, warmup):
     return t.item() / steps
 
 
-def load_json(path):
-    try:
-        return json.load(open(path))
-    except Exception:
-        return None
-
-
 def roofline_of(workload, stats, rows, peak, peak_src):
     launches = max(1, stats["hot_launches"])
     alg = ALG_BYTES_PER_ROW[workload]
     achieved = alg * stats["hot_rows"] / max(1, stats["hot_ns"])                  # bytes/ns == GB/s
     launch_rows = min(rows, LAUNCH_ROWS)
-    traffic, traffic_src = None, None
-    tj = load_json(os.path.join(ROOT, "profiles", "r02_traffic.json")) or {}
-    ent = tj.get(workload)
-    if ent and ent.get("rows_per_launch") == launch_rows:                           # DRAM bytes of ONE launch of the same kernel at the same rows/launch
-        traffic, traffic_src = ent["dram_bytes_read"] + ent["dram_bytes_write"], ent.get("source")
     return {"bound": "hbm", "achieved": achieved, "peak": peak, "peak_source": peak_src, "unit": "GB/s", "frac": achieved / peak,
-            "traffic": traffic, "traffic_source": traffic_src, "kernel": {"M2": "agg_tile_dense_kernel<2,1,2,1>", "M1": "agg_lean_dense_kernel<2,2,1>", "M0": "filter_count_lean + filter_apply_lean (two-pass compaction)"}[workload],
+            "kernel": {"M2": "agg_tile_dense_kernel<2,1,2,1>", "M1": "agg_lean_dense_kernel<2,2,1>", "M0": "filter_count_lean + filter_apply_lean (two-pass compaction)"}[workload],
             "launches": stats["hot_launches"], "avg_launch_ms": stats["hot_ns"] / launches / 1e6, "launch_rows": launch_rows,
             "alg_bytes_per_row": alg, "alg_bytes_per_launch": alg * launch_rows}
 
@@ -498,9 +508,7 @@ def run_ours(args):
         exchange = native.Exchange(bytes(uid.cpu().numpy().tobytes()), rank, world, local)
     rows = env_int("B200Q_BENCH_ROWS", 1_000_000_000)
     extra_rows = env_int("B200Q_BENCH_EXTRA_ROWS", rows)
-    peaks = load_json(os.path.join(ROOT, "MEASURED_PEAKS.json")) or {}
-    peak_src = "measured" if "hbm_gbs" in peaks else "fallback"
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak, peak_src = HBM_PEAK_GBS, "H100 SXM data sheet"
     failures = []
 
     # ---- headline: M2 -------------------------------------------------------------------------------------------
@@ -519,6 +527,8 @@ def run_ours(args):
     if not ok:
         failures.append("M2")
     verified = {"M2": dict(ok=ok, **info)}
+    if args.dump_outputs:
+        r2.dump(args.dump_outputs)
 
     # ---- e2e: host buffers through the C ABI (M2) -------------------------------------------------------------------
     import numpy as np
@@ -546,14 +556,14 @@ def run_ours(args):
             out.append(pa.RecordBatch.from_arrays(arrs, schema=schema))
         return out
     hb = host_batches(host, e2e_rows, e2e_batch)
-    e2e_steps = max(1, min(args.steps, 5))
+    e2e_steps = args.steps
     ms_e2e = timed(torch, dist, world, dev, lambda: r2.step_host(hb), e2e_steps, max(1, min(args.warmup, 2)))
     e2e = {"value": e2e_rows * world / (ms_e2e * 1e-3), "unit": "rows/s", "h2d_bytes_per_step": r2.h2d, "d2h_bytes_per_step": r2.d2h,
            "rows_per_gpu": e2e_rows, "host_batch_rows": e2e_batch, "host_memory": "pinned", "steps": e2e_steps, "host_numa_node": numa}
     # 10,000-row pageable batches: the shape FFIReaderExec really hands over (<= BATCH_SIZE rows, ordinary heap memory)
     small_rows = int(min(e2e_rows, env_int("B200Q_BENCH_E2E_SMALL_ROWS", 1 << 26)))
     hb_small = host_batches(host, small_rows, 10000, copy=True)
-    ms_small = timed(torch, dist, world, dev, lambda: r2.step_host(hb_small), max(1, min(args.steps, 3)), 1)
+    ms_small = timed(torch, dist, world, dev, lambda: r2.step_host(hb_small), args.steps, 1)
     e2e["pageable_10k"] = {"value": small_rows * world / (ms_small * 1e-3), "unit": "rows/s", "h2d_bytes_per_step": r2.h2d, "d2h_bytes_per_step": r2.d2h,
                            "rows_per_gpu": small_rows, "host_batch_rows": 10000, "host_memory": "pageable, staged into the library's pinned ring (staging_rows = 2^20)"}
     del hb_small
@@ -570,7 +580,7 @@ def run_ours(args):
 
     # ---- extras: M1 and M0, each timed, verified and with its own roofline ------------------------------------------
     extra = []
-    ex_steps, ex_warm = max(1, min(args.steps, 10)), max(3, min(args.warmup, 3))
+    ex_steps, ex_warm = args.steps, 3
     for w in ("M1", "M0"):
         r = Runner(w, torch, dist, native, rank, world, local, extra_rows, exchange)
         for _ in range(ex_warm):
@@ -587,7 +597,7 @@ def run_ours(args):
         torch.cuda.empty_cache()
 
     x_rows = env_int("B200Q_BENCH_X_ROWS", min(extra_rows, 1 << 28))
-    xs, ok3, ok4 = extra_shuffle_and_join(torch, dist, native, world, local, dev, x_rows, max(1, min(args.steps, 5)), 3, peak, peak_src, 48 + 1000 * rank)
+    xs, ok3, ok4 = extra_shuffle_and_join(torch, dist, native, world, local, dev, x_rows, args.steps, 3, peak, peak_src, 48 + 1000 * rank)
     extra += xs
     verified["M3"], verified["M4"] = {"ok": ok3}, {"ok": ok4}
     if not ok3: failures.append("M3")
@@ -604,7 +614,7 @@ def run_ours(args):
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "int64", "data": "synthetic",
             "config": {"workload": WORKLOADS["M2"], "rows_per_gpu": rows, "groups": CARD,
                        "parallelism": f"dp{world}" + ("" if world == 1 else " + murmur3(42) pmod N ownership, in-library NCCL AllToAllv of the columnar partial states (b200q_exchange_shuffle)"),
-                       "l2_policy": "input (%.1f GB/GPU) is far larger than the 126 MB L2; no flush needed" % (rows * 32 / 1e9),
+                       "l2_policy": "input (%.1f GB/GPU) is far larger than the 50 MB L2; no flush needed" % (rows * 32 / 1e9),
                        "plan": "FilterExec fused into AggExec(Partial) -> AggExec(Final), reference protobuf + C ABI"},
             "e2e": e2e, "gpu_launches": headline_stats["launches"], "clocks": clocks,
             "roofline": roofline_of("M2", headline_stats, rows, peak, peak_src), "cpu_baseline": cpu, "verified": verified, "extra": extra,
@@ -669,7 +679,7 @@ def cpu_model():
 
 def thread_candidates():
     """the restatement builds one full group table per task, so its merge grows with the task count and it does NOT scale
-    to every core (profiles/r01_cpu_ref_thread_scaling.txt): time a few thread counts and report the best"""
+    to every core (tools/cpu_scaling.py): time a few thread counts and report the best"""
     top = usable_cores()
     return sorted({t for t in (8, 16, 32, top) if 1 <= t <= top} or {top})
 
@@ -729,6 +739,7 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed M2 step's result columns to DIR/*.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -514,7 +514,7 @@ static void conf_defaults(b200q_conf* c) {
   c->partial_state_columnar = 0;
   c->force_generic_kernels = 0;
   c->agg_dense_keys = 1;
-  c->agg_hot_key_cache = 1;                            // skew probe on the first batch -> CTA-private hot-key cache (validated on B200 in round 2)
+  c->agg_hot_key_cache = 1;                            // skew probe on the first batch -> CTA-private hot-key cache
 }
 
 }  // namespace b200q
@@ -528,7 +528,7 @@ static void conf_defaults(b200q_conf* c) {
 extern "C" {
 
 int32_t b200q_version(void) { return 100; }
-const char* b200q_build_info(void) { return "blaze_b200 hot path: Filter/Project/HashAgg, sm_100a, CUDA " B200Q_STR(CUDART_VERSION); }
+const char* b200q_build_info(void) { return "blaze_b200 hot path: Filter/Project/HashAgg, sm_90a, CUDA " B200Q_STR(CUDART_VERSION); }
 const char* b200q_last_error(void) { return g_last_error.c_str(); }
 int32_t b200q_device_count(void) { int n = 0; if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; } return n; }
 
@@ -554,7 +554,7 @@ b200q_status b200q_op_create(const uint8_t* plan, size_t plan_len, int32_t plan_
   b200q_status st = guarded(nullptr, [&] {
     PlanP p = decode_plan(plan, plan_len, plan_kind);
     int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); throw ExecError(B200Q_ERR_NO_DEVICE, "no CUDA device is visible: the sm_100a kernels cannot run and there is no CPU fallback"); }
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); throw ExecError(B200Q_ERR_NO_DEVICE, "no CUDA device is visible: the sm_90a kernels cannot run and there is no CPU fallback"); }
     if (device < 0 || device >= ndev) throw ExecError(B200Q_ERR_INVALID_ARG, "invalid device ordinal");
     op = new b200q_op();
     op->plan = p; op->cx.device = device;

@@ -90,7 +90,7 @@ __global__ void __launch_bounds__(PT_BLOCK) scatter_bits_kernel(const uint8_t* _
 }
 
 static int pt_grid(int64_t n, int per_block) {
-  int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t want = (n + per_block - 1) / per_block, cap = (int64_t)sms * 8;
   return (int)std::max<int64_t>(1, std::min(want, cap));
 }

@@ -1,7 +1,7 @@
 // Hash join stages (SURVEY.md §8(f) rank 2): JoinBuildStage (BroadcastJoinBuildHashMapExecNode) and JoinProbeStage
 // (BroadcastJoinExecNode / HashJoinExecNode).
 //
-// Reference (paths relative to /root/reference/native-engine/datafusion-ext-plans/src/):
+// Reference (paths relative to the reference's native-engine/datafusion-ext-plans/src/):
 //   BroadcastJoinBuildHashMapExec::execute    broadcast_join_build_hash_map_exec.rs:148-236 (collect the side, build ONE map)
 //   BroadcastJoinExec::execute / execute_join broadcast_join_exec.rs:226-298, 496-560 (map side = broadcast / build side; the
 //                                             other child is streamed through a Joiner)

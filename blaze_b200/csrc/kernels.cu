@@ -1,4 +1,4 @@
-// Hand-written sm_100a kernels of the Filter / Project / HashAgg hot path (generic, VM-driven forms;
+// Hand-written sm_90a kernels of the Filter / Project / HashAgg hot path (generic, VM-driven forms;
 // the specialised streaming kernels live in kernels_fast.cu).
 //
 //   filter_project_kernel  K1+K2+K3 of SURVEY.md §2.4 fused: predicate mask, ordered stream compaction
@@ -163,7 +163,7 @@ int launch_filter_project(const VmProgram* d_prog, const ColTable& cols, const O
   (void)nouts;
   const int64_t ntiles = filter_project_num_tiles(n);
   if (ntiles == 0) return 0;
-  int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t grid = ntiles < (int64_t)sms * 8 ? ntiles : (int64_t)sms * 8;     // persistent: a multiple of the SM count
   filter_project_kernel<<<(unsigned)grid, FP_BLOCK, 0, s>>>(d_prog, cols, outs, n, ntiles, has_filters ? 1 : 0, d_tile_status, d_scratch);
   return 1;
@@ -175,10 +175,9 @@ static int grid_for(int64_t ntiles, int per_sm);
 // lean FilterExec / ProjectExec for the M0 shape: 1-4 non-null int64 input columns, `col cmp literal` conjuncts,
 // projections that are a column or `column op column|literal`; expressions evaluated directly (no bytecode).
 //
-// Measured on B200 (profiles/r01_filter_lookback_phases.txt): in the single-pass look-back form a tile spends 65 %
-// of its life WAITING for its exclusive prefix (7.4 us of 11.4 us at 2048-row tiles) with its rows parked in
-// registers and no loads in flight; wider windows, larger tiles, back-off and earlier tickets all end at
-// 1.1-1.3e11 rows/s (0.39-0.44 of the HBM roofline).  Large batches therefore take an order-free two-pass form:
+// In the single-pass look-back form a tile spends most of its life WAITING for its exclusive prefix with its rows
+// parked in registers and no loads in flight; wider windows, larger tiles, back-off and earlier tickets do not
+// change that.  Large batches therefore take an order-free two-pass form:
 //   pass 1  count : every warp streams the FILTER columns of its 256-row chunks and writes one survivor count
 //   (scan)        : exclusive scan of the chunk counts (3 tiny launches)
 //   pass 2  apply : every warp streams all referenced columns of its chunks, re-evaluates the conjuncts and
@@ -483,17 +482,16 @@ int launch_filter_project_lean(const ColTable& cols, int ncols, const LeanFpSpec
     d.out[o].lit = sp.out[o].lit; d.out[o].dst = out_values[o];
   }
 #ifndef B200Q_EMULATED_DEVICE
-  {   // large batches: the TMA-staged single pass exists (B200Q_FILTER_TMA=1) but is NOT the default: measured on B200 at 2^28 rows it runs at
-      // 1.12e11 rows/s (0.41 of the HBM peak) against 1.78e11 (0.65) for the two-pass form — with a fully resident grid walking the tiles in
-      // lockstep, every tile's look-back has to sum the aggregates of a whole wave (~440 tiles, 14 dependent L2 round trips) while a tile is only
-      // ~2 us of HBM time; the two-pass form already moves its 32 B/row at 87 % of the copy bandwidth (profiles/r02_shapes_m0_*.txt)
+  {   // large batches: the TMA-staged single pass exists (B200Q_FILTER_TMA=1) but is NOT the default: with a fully resident grid walking the
+      // tiles in lockstep, every tile's look-back has to sum the aggregates of a whole wave (hundreds of tiles, a chain of dependent L2
+      // round trips) while a tile is only microseconds of HBM time; the two-pass form streams both passes at HBM speed
     static const bool two_pass = getenv("B200Q_FILTER_TMA") == nullptr;
     bool aligned = true;
     for (int c = 0; c < ncols; c++) aligned = aligned && (((uintptr_t)d.col[c]) & 15) == 0;
     if (!two_pass && aligned && sp.nfilt && n >= FL_TWO_PASS_MIN_ROWS) {
       const int64_t ntiles = (n + FL_TILE - 1) / FL_TILE;
       const size_t smem = (size_t)2 * ncols * FL_TILE * 8;
-      int occ = 0, dev = 0, sms = 148;
+      int occ = 0, dev = 0, sms = 132;
       cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
 #define B200Q_FTMA(NC_) do { cudaFuncSetAttribute(filter_project_tma_kernel<NC_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, filter_project_tma_kernel<NC_>, FL_BLOCK, smem); \
@@ -654,7 +652,7 @@ __global__ void __launch_bounds__(AG_BLOCK) agg_update_kernel(const VmProgram* _
 }
 
 static int grid_for(int64_t ntiles, int per_sm) {
-  int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t cap = (int64_t)sms * per_sm;       // grid = multiple of the SM count (persistent, grid-stride)
   return (int)(ntiles < cap ? (ntiles < 1 ? 1 : ntiles) : cap);
 }

@@ -31,9 +31,9 @@ struct AccOp {
   uint8_t arg_out[4];  // VM output index of each argument
 };
 
-// The table is split in two arrays indexed by the slot number (measured on B200, profiles/r01_microbench_probe_*:
-// a probe load followed by a RED on the SAME sector runs at 5.2e10 rows/s, probing one array and RED-ing another
-// at 1.0e11 — the L2s of the two dies keep read copies that every atomic on the line must invalidate):
+// The table is split in two arrays indexed by the slot number (tools/microbench/probes.cu compares the layouts: a probe
+// load followed by a RED on the SAME sector is slower than probing one array and RED-ing another, because the read
+// copies the L2 keeps of a line must be invalidated by every atomic on it):
 //   key entry  = [hdr][key words...]           kstride words, probed with plain loads, written once at insertion
 //   acc entry  = [accumulator words...]        astride words, only ever touched by RED/ATOM
 //   hdr low 32 bits : tag  (0 empty, 1 locked, else 0x80000000|fingerprint — cf. agg_hash_map.rs:228-234)

@@ -3,9 +3,9 @@
 //   * up to 4 fused `column <cmp> literal` conjuncts (the FilterExec below the agg),
 //   * 1-2 accumulators of the "64-bit add" class: SUM(int column), COUNT(column), COUNT(*).
 //
-// What bounds them (profiles/r01_microbench_*.txt, measured on B200): the input stream runs at HBM speed
-// (6.5 TB/s) but every row also needs a random read-modify-write into the L2-resident group table, and the chip
-// retires ~1.55e11 scattered 32-byte RED sector operations per second.  So the design goal is ONE RED sector per row:
+// What bounds them (tools/microbench/atomics.cu measures it): the input stream runs at HBM speed but every row also
+// needs a random read-modify-write into the L2-resident group table, and the chip retires a bounded number of
+// scattered 32-byte RED sector operations per second.  So the design goal is ONE RED sector per row:
 //   - hashed (agg_lean_hash_kernel): key entries {hdr,key..} and accumulator entries live in two arrays (a RED on a
 //     sector that was just probed costs 2x: the read copies must be invalidated); the probe is a single 16-byte
 //     load, collided rows are re-probed 32 at a time from a per-warp stack, and the two accumulators of a row are
@@ -82,10 +82,11 @@ __device__ __forceinline__ bool dense_index(const FastSpec& fs, long long k0, lo
 // Per 32 rows a warp issues 1 (+1) wide streaming loads and G REDG: ~2 instructions per row.
 // ---------------------------------------------------------------------------------------------------
 template <int G> struct i64xG { long long v[G]; };
-__device__ __forceinline__ i64xG<4> ld_stream_vec(const long long* p, i64xG<4>*) {
-  i64xG<4> r;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v4.b64 {%0,%1,%2,%3}, [%4];"
-               : "=l"(r.v[0]), "=l"(r.v[1]), "=l"(r.v[2]), "=l"(r.v[3]) : "l"(p));
+__device__ __forceinline__ i64xG<4> ld_stream_vec(const long long* p, i64xG<4>*) {     // two 128-bit loads: the widest on sm_90
+  i64xG<4> r; uint64_t pol;
+  asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));                // not volatile: hoisted out of the loop
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0,%1}, [%4], %5;\n\tld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%2,%3}, [%4+16], %5;"
+               : "=l"(r.v[0]), "=l"(r.v[1]), "=l"(r.v[2]), "=l"(r.v[3]) : "l"(p), "l"(pol));
   return r;
 }
 __device__ __forceinline__ i64xG<2> ld_stream_vec(const long long* p, i64xG<2>*) {
@@ -724,7 +725,7 @@ __global__ void __launch_bounds__(FA_BLOCK) agg_dense_smem_kernel(const ColTable
 }
 
 static int fast_grid(int64_t ntiles) {
-  int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t cap = (int64_t)sms * 8;          // persistent grid: a multiple of the SM count
   return (int)(ntiles < cap ? (ntiles < 1 ? 1 : ntiles) : cap);
 }

@@ -1,6 +1,6 @@
 // Hash join on the GPU (SURVEY.md §8(f) rank 2): build + probe + gather kernels of JoinBuildStage / JoinProbeStage.
 //
-// Reference (paths relative to /root/reference/native-engine/datafusion-ext-plans/src/):
+// Reference (paths relative to the reference's native-engine/datafusion-ext-plans/src/):
 //   Table::create_from_key_columns, lookup_many      joins/join_hash_map.rs:105-275
 //   FullJoiner::join / finish                        joins/bhj/full_join.rs:209-362
 //   SemiJoiner::join / finish                        joins/bhj/semi_join.rs:146-312
@@ -28,7 +28,7 @@ constexpr int JB = 256;
 #endif
 
 int jgrid(int64_t n, int per_block = JB * 4) {
-  int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return (int)std::max<int64_t>(1, std::min<int64_t>((n + per_block - 1) / per_block, (int64_t)sms * 8));
 }
 

@@ -17,7 +17,7 @@ namespace {
 
 constexpr int PB = 256;
 int pgrid(int64_t n) {
-  int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return (int)std::max<int64_t>(1, std::min<int64_t>((n + PB * 4 - 1) / (PB * 4), (int64_t)sms * 8));
 }
 

@@ -32,7 +32,7 @@ __device__ __forceinline__ uint32_t sh_mix_h1(uint32_t h1, uint32_t k1) { h1 ^= 
 __device__ __forceinline__ uint32_t sh_fmix(uint32_t h1, uint32_t len) { h1 ^= len; h1 ^= h1 >> 16; h1 *= 0x85ebca6bu; h1 ^= h1 >> 13; h1 *= 0xc2b2ae35u; h1 ^= h1 >> 16; return h1; }
 
 int sm_count() {
-  int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return sms;
 }
 
@@ -356,9 +356,10 @@ int launch_shuffle_encode(const ShufSpec& sp, const uint16_t* d_pids, int64_t n,
   ShufSpec spx = sp;
   bool tma = false;
 #ifndef B200Q_EMULATED_DEVICE
-  // measured on B200 (profiles/r02_shapes_shuffle_*): the bulk-copy staging costs 64 KB more shared memory per CTA (a smaller L1 for the
-  // write-combining of the byte stores) and the kernel is bound by its store phase, not by the column loads: off unless asked for
-  static const bool no_tma = getenv("B200Q_SHUFFLE_TMA") == nullptr;
+  // the bulk-copy staging costs 64 KB more shared memory per CTA (a smaller L1 for the write-combining of the byte stores) but takes
+  // the column loads off the warps' critical path; on H100 it is the faster form (bench.py M3, 200-way, 2^28 rows: 26.7 ms against
+  // 30.4-31.2 ms per step, H100 SXM 80 GB at 700 W), so it is the default; B200Q_SHUFFLE_TMA=0 selects the register-staged form
+  static const bool no_tma = [] { const char* e = getenv("B200Q_SHUFFLE_TMA"); return e != nullptr && e[0] == '0'; }();
   for (int c = 0; c < spx.ncols; c++) {                                                     // bulk copies need 16-byte aligned sources
     ShufCol& col = spx.col[c];
     col.tma = !no_tma && (col.width == 1 || col.width == 2 || col.width == 4 || col.width == 8) && ((uintptr_t)col.values & 15) == 0 && n >= SHUF_TILE;

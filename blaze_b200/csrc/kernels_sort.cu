@@ -24,7 +24,7 @@ namespace {
 constexpr int SB = 256, S_ITEMS = 16, S_TILE = SB * S_ITEMS, S_WARPS = SB / 32;
 
 int sgrid(int64_t n, int per_block = SB * 4) {
-  int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return (int)std::max<int64_t>(1, std::min<int64_t>((n + per_block - 1) / per_block, (int64_t)sms * 8));
 }
 

@@ -3,9 +3,9 @@
 //
 // Why: the one-row-per-lane kernels of kernels_fast.cu issue one 8-byte (or narrower) load per row per column plus one
 // validity-byte load per row, re-read a filter column once per conjunct, and run G shuffle + RED steps per 32 rows
-// whether or not the rows survived the filter (profiles/r02_ncu_baseline_*.txt: M2 0.44 of HBM peak, typed 0.12).
+// whether or not the rows survived the filter.
 // Here a warp owns a TILE of 128 consecutive rows and every lane 4 consecutive rows of it:
-//   * one vector load per column per lane (256-bit for int64, 128-bit for int32, 64/32-bit for int16/int8) and ONE
+//   * one 32-byte run per column per lane (two 128-bit loads for int64, one 128-bit for int32, 64/32-bit for int16/int8) and ONE
 //     validity nibble per column per lane (a 32-lane load covers 128 validity bits);
 //   * the conjuncts on one column are merged on the host into one closed interval [lo, hi] (FilterExec conjuncts are
 //     pre-split `col cmp literal` terms, NativeFilterBase.scala:66-87), tested with one subtract + one unsigned compare;
@@ -30,8 +30,10 @@ constexpr int TL_BLOCK = 256, TL_WARPS = TL_BLOCK / 32, TL_ROWS = 128;
 __device__ __forceinline__ uint64_t tl_policy_evict_first() {
   uint64_t pol; asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol)); return pol;
 }
-__device__ __forceinline__ void tl_ld_v4b64(const long long* p, long long (&v)[4]) {
-  asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v4.b64 {%0,%1,%2,%3}, [%4];" : "=l"(v[0]), "=l"(v[1]), "=l"(v[2]), "=l"(v[3]) : "l"(p));
+// 4 consecutive int64 as two 128-bit loads (the widest a thread can issue on sm_90); p is 16-byte aligned
+__device__ __forceinline__ void tl_ld_v4b64(const long long* p, uint64_t pol, long long (&v)[4]) {
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0,%1}, [%4], %5;\n\tld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%2,%3}, [%4+16], %5;"
+               : "=l"(v[0]), "=l"(v[1]), "=l"(v[2]), "=l"(v[3]) : "l"(p), "l"(pol));
 }
 __device__ __forceinline__ long long tl_ld_b64(const long long* p, uint64_t pol) {
   long long v; asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.b64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol)); return v;
@@ -65,7 +67,7 @@ __device__ __forceinline__ void tl_load4(const DevCol& c, int phys, long long ro
   switch (phys) {
     case PH_I64: {
       const long long* p = (const long long*)c.values + row0;
-      if (nrow == 4 && ((uintptr_t)p & 31) == 0) tl_ld_v4b64(p, v);
+      if (nrow == 4 && ((uintptr_t)p & 15) == 0) tl_ld_v4b64(p, pol, v);
       else {
 #pragma unroll
         for (int j = 0; j < 4; j++) if (j < nrow) v[j] = tl_ld_b64(p + j, pol);
@@ -127,7 +129,7 @@ __global__ void __launch_bounds__(TL_BLOCK) agg_tile_dense_kernel(const ColTable
   const long long ntiles = (n + TL_ROWS - 1) / TL_ROWS;
   const bool add0 = fs.acc[0].kind == FAST_ACC_ADD, add1 = NACC == 2 && fs.acc[1].kind == FAST_ACC_ADD;
   // this lane's entry word as branch-free selectors (the G lanes of a group hold G different word kinds: a switch
-  // here is a 4-way divergent branch in the innermost loop — r02_ncu_tile_dense_v1: 16 of 32 threads active, 14 instr/row):
+  // here is a 4-way divergent branch in the innermost loop):
   //   val = c_one + (v0 & m0) + (v1 & m1) + ((pk >> vshift) & mvalid)
   unsigned long long c_one = 0, m0 = 0, m1 = 0; unsigned vshift = 28, mvalid = 0;
   {
@@ -224,7 +226,7 @@ __global__ void __launch_bounds__(TL_BLOCK) agg_tile_dense_kernel(const ColTable
 }
 
 static int tile_grid(int64_t ntiles, int ctas_per_sm) {
-  int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t want = (ntiles + TL_WARPS - 1) / TL_WARPS, cap = (int64_t)sms * ctas_per_sm;      // persistent grid: a multiple of the SM count
   return (int)std::max<int64_t>(1, std::min(want, cap));
 }
@@ -254,7 +256,7 @@ template <int FLAV> __device__ __forceinline__ void tw_red(unsigned long long* p
 }
 template <int FLAV> __device__ __forceinline__ unsigned long long tw_noop() { return FLAV == TF_MIN_S64 ? 0x7FFFFFFFFFFFFFFFULL : 0ULL; }
 
-// the 4 rows of one decimal128 column: low and high words (two 256-bit loads per lane)
+// the 4 rows of one decimal128 column: low and high words (four 128-bit loads per lane)
 __device__ __forceinline__ void tl_load4_dec(const DevCol& c, long long row0, int nrow, uint64_t pol, long long (&lo)[4], long long (&hi)[4], unsigned& valid) {
   valid = (1u << nrow) - 1u;
   if (c.validity && nrow > 0) valid &= tl_nibble(c.validity, (unsigned long long)row0 + c.bit_offset, nrow);
@@ -262,8 +264,8 @@ __device__ __forceinline__ void tl_load4_dec(const DevCol& c, long long row0, in
   for (int j = 0; j < 4; j++) { lo[j] = 0; hi[j] = 0; }
   if (nrow <= 0) return;
   const long long* p = (const long long*)c.values + 2 * row0;
-  if (nrow == 4 && ((uintptr_t)p & 31) == 0) {
-    long long a[4], b[4]; tl_ld_v4b64(p, a); tl_ld_v4b64(p + 4, b);
+  if (nrow == 4 && ((uintptr_t)p & 15) == 0) {
+    long long a[4], b[4]; tl_ld_v4b64(p, pol, a); tl_ld_v4b64(p + 4, pol, b);
     lo[0] = a[0]; hi[0] = a[1]; lo[1] = a[2]; hi[1] = a[3]; lo[2] = b[0]; hi[2] = b[1]; lo[3] = b[2]; hi[3] = b[3];
   } else {
 #pragma unroll

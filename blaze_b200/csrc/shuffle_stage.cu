@@ -1,6 +1,6 @@
 // ShuffleWriteStage: the terminal stage of a plan rooted at ShuffleWriterExecNode (SURVEY.md §8(f) rank 1).
 //
-// Reference behaviour restated (paths relative to /root/reference/native-engine/datafusion-ext-plans/src/):
+// Reference behaviour restated (paths relative to the reference's native-engine/datafusion-ext-plans/src/):
 //   ShuffleWriterExec::execute            shuffle_writer_exec.rs:109-165   (repartitioner by partitioning kind; empty output stream)
 //   SortShuffleRepartitioner              shuffle/sort_repartitioner.rs:121-185 (insert_batch -> BufferedData; shuffle_write: .data + .index)
 //   BufferedData::write                   shuffle/buffered_data.rs:123-158 (per partition: batches -> IpcCompressionWriter, finish_current_buf)

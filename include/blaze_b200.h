@@ -1,5 +1,5 @@
 /*
- * blaze_b200.h — C ABI of the B200-native Filter / Project / HashAgg hot path.
+ * blaze_b200.h — C ABI of the H100-native Filter / Project / HashAgg hot path.
  *
  * This is the drop-in boundary posited by BASELINE.json's north_star: the reference
  * (kwai/blaze = Apache Auron @ d1eaef148a58) keeps its Rust host code — plan-serde, JNI bridge,
@@ -7,7 +7,7 @@
  * points instead of running the CPU operator.  INTEGRATION.md shows the Rust shim.
  *
  * Every entry point names the reference interface it replaces (paths relative to
- * /root/reference/native-engine/):
+ * the reference's native-engine/):
  *
  *   b200q_op_create         FilterExec::try_new   datafusion-ext-plans/src/filter_exec.rs:51-73
  *                           ProjectExec::try_new  datafusion-ext-plans/src/project_exec.rs:57-81
@@ -115,7 +115,7 @@ typedef int32_t b200q_status;
 #define B200Q_ERR_CUDA 3         /* CUDA runtime failure; sticky for the handle                    */
 #define B200Q_ERR_STATE 4        /* call sequence violation (push after finish, ...)               */
 #define B200Q_ERR_EXECUTION 5    /* data-dependent error, e.g. "Divide by zero error"              */
-#define B200Q_ERR_NO_DEVICE 6    /* no CUDA device / sm_100a kernels cannot run: NEVER falls back   */
+#define B200Q_ERR_NO_DEVICE 6    /* no CUDA device / sm_90a kernels cannot run: NEVER falls back    */
 #define B200Q_ERR_INVALID_ARG 7
 
 /* plan_kind for b200q_op_create / b200q_plan_explain */

@@ -3,7 +3,7 @@
 A numpy restatement of the reference's Filter / Project / HashAgg semantics
 (kwai/blaze = Apache Auron @ d1eaef148a58), used by `tests/`, `__graft_entry__.smoke()` and
 `bench.py`'s cpu_baseline leg as the checker for the CUDA path.  Each function cites the
-reference file:line it follows (paths relative to /root/reference/native-engine/).
+reference file:line it follows (paths relative to the reference's native-engine/).
 
 PARITY STATUS
   * HashAgg (Sum/Count/Avg/Min/Max, Partial/PartialMerge/Final, frozen-row bytes, varint):

@@ -1,7 +1,7 @@
 """CPU restatement of the reference's hash join (BroadcastJoinExec / HashJoinExec, SURVEY.md §8(f) rank 2) — TEST
 INFRASTRUCTURE ONLY (tests/, smoke and bench's cpu_baseline may import it; the product never does).
 
-Paths relative to /root/reference/native-engine/datafusion-ext-plans/src/:
+Paths relative to the reference's native-engine/datafusion-ext-plans/src/:
   JoinHashMap / Table::create_from_key_columns / lookup_many      joins/join_hash_map.rs:91-275 (rows whose key has a NULL
                                                                   are left out of the map :119-128; duplicates of a key sit in
                                                                   one `mapped_indices` range in row order :129-143)

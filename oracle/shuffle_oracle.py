@@ -2,7 +2,7 @@
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg may import this module; the product
 (blaze_b200/) never does.  Every function cites the reference file:line it follows (paths relative to
-/root/reference/native-engine/).
+the reference's native-engine/).
 
   radix_sort_by_key                datafusion-ext-commons/src/algorithm/rdx_sort.rs:23-73   (unstable American-flag sort)
   evaluate_*_partition_ids         datafusion-ext-plans/src/shuffle/mod.rs:163-275

@@ -24,7 +24,7 @@ def test_every_declared_symbol_is_exported():
 
 def test_identity_calls_work_without_gpu():
     assert native.lib.b200q_version() >= 100
-    assert b"sm_100a" in native.lib.b200q_build_info()
+    assert b"sm_90a" in native.lib.b200q_build_info()
     assert native.device_count() >= 0
     c = native.default_conf()
     assert c.batch_size == 10000 and c.suggested_batch_mem_size == 8388608          # commons/src/lib.rs:74-82

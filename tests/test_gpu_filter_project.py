@@ -166,7 +166,7 @@ def test_lean_project_only_and_filter_only():
 @pytest.mark.parametrize("n", [1 << 20, 3_000_037])
 def test_lean_large_batch_forms(n):
     """batches of >= 2^20 rows take the order-free count / scan / apply form (or, with B200Q_FILTER_TMA=1, the TMA-staged single pass:
-    cp.async.bulk tiles + decoupled look-back over a fully resident grid — validated on B200 but slower, see kernels.cu): ragged last
+    cp.async.bulk tiles + decoupled look-back over a fully resident grid — bit-exact but not faster, see kernels.cu): ragged last
     tile, 3 input columns, conjuncts on two of them, every selectivity regime inside one batch (sorted run + random part)"""
     rng = np.random.default_rng(n)
     a = rng.integers(0, 1000, n, dtype=np.int64); a[: n // 4] = np.sort(a[: n // 4])

@@ -1,6 +1,5 @@
 """Skewed keys: the skew probe on the first batch selects the CTA-private hot-key cache kernel
-(b200q_conf.agg_hot_key_cache, on by default since it was validated on B200 in round 2:
-profiles/r02_skew_hot_key_cache.txt, Zipf(1.1) 1.48e10 -> 1.13e11 rows/s)."""
+(b200q_conf.agg_hot_key_cache, on by default)."""
 import os
 
 import numpy as np

@@ -1,38 +1,22 @@
-"""blaze_b200/proto.py declares the hot-path subset of the reference's auron.proto programmatically;
-when the reference is mounted, every message/field/number/type is checked against the .proto text."""
+"""blaze_b200/proto.py declares the hot-path subset of the reference's auron.proto programmatically; every
+message/field/number/type is checked against the reference's field table stored in tests/golden/auron_proto_fields.json
+(extracted from auron.proto of kwai/blaze @ d1eaef148a58)."""
+import json
 import os
-import re
-
-import pytest
 
 from blaze_b200 import proto as P
 
-REF = "/root/reference/native-engine/auron-serde/proto/auron.proto"
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "auron_proto_fields.json")
 
 
-def _parse_reference():
-    text = re.sub(r"//.*", "", open(REF).read())
-    msgs = {}
-    for m in re.finditer(r"message\s+(\w+)\s*\{", text):
-        name, i, depth = m.group(1), m.end(), 1
-        j = i
-        while depth:
-            depth += {"{": 1, "}": -1}.get(text[j], 0)
-            j += 1
-        body = text[i:j - 1]
-        fields = {}
-        for f in re.finditer(r"(repeated\s+)?([\w.]+)\s+(\w+)\s*=\s*(\d+)\s*;", body):
-            fields[f.group(3)] = (int(f.group(4)), f.group(2), bool(f.group(1)))
-        msgs[name] = fields
-    enums = {}
-    for m in re.finditer(r"enum\s+(\w+)\s*\{([^}]*)\}", text):
-        enums[m.group(1)] = {a: int(b) for a, b in re.findall(r"(\w+)\s*=\s*(\d+)\s*;", m.group(2))}
-    return msgs, enums
+def _reference_tables():
+    g = json.load(open(GOLDEN))
+    msgs = {m: {f: (num, typ, rep) for f, (num, typ, rep) in fields.items()} for m, fields in g["messages"].items()}
+    return msgs, g["enums"]
 
 
-@pytest.mark.skipif(not os.path.exists(REF), reason="reference not mounted")
 def test_field_numbers_match_reference_proto():
-    msgs, enums = _parse_reference()
+    msgs, enums = _reference_tables()
     from google.protobuf import descriptor_pb2 as dpb
     F = dpb.FieldDescriptorProto
     scalar = {F.TYPE_STRING: "string", F.TYPE_BYTES: "bytes", F.TYPE_BOOL: "bool", F.TYPE_UINT32: "uint32",

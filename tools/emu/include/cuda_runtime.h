@@ -85,7 +85,7 @@ inline double __ll2double_rn(long long v) { return (double)v; }
 inline float __ll2float_rn(long long v) { return (float)v; }
 inline float __double2float_rn(double v) { return (float)v; }
 inline long long __double2ll_rn(double v) { return (long long)nearbyint(v); }
-inline long long __double2ll_rz(double v) { return v != v ? INT64_MIN /* cvt.rzi.s64.f64 maps NaN to 0x8000000000000000 (seen on B200) */ : v >= 9223372036854775807.0 ? INT64_MAX : v <= -9223372036854775808.0 ? INT64_MIN : (long long)v; }
+inline long long __double2ll_rz(double v) { return v != v ? INT64_MIN /* cvt.rzi.s64.f64 maps NaN to 0x8000000000000000 (what the device conversion returns) */ : v >= 9223372036854775807.0 ? INT64_MAX : v <= -9223372036854775808.0 ? INT64_MIN : (long long)v; }
 inline float __fadd_rn(float a, float b) { return a + b; }
 inline float __fsub_rn(float a, float b) { return a - b; }
 inline float __fmul_rn(float a, float b) { return a * b; }

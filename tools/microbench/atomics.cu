@@ -1,6 +1,6 @@
-// Microbenchmark: how fast can a B200 do "random RMW into an L2-resident group table" ?
+// Microbenchmark: how fast can an H100 do "random RMW into an L2-resident group table" ?
 // Decides the HashAgg slot layout (SoA vs AoS, paired lanes, probe + RED).
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o atomics atomics.cu
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o atomics atomics.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>
@@ -96,10 +96,10 @@ int main(int argc,char**argv){
   int64_t *k,*v; CK(cudaMalloc(&k,n*8)); CK(cudaMalloc(&v,n*8));
   size_t slots = 1; while(slots < card*2) slots<<=1;          // load <= 0.5
   size_t tbytes = slots*32; unsigned long long *t0,*t1,*sink; CK(cudaMalloc(&t0,tbytes)); CK(cudaMalloc(&t1,tbytes)); CK(cudaMalloc(&sink,8));
-  gen<<<148*8,256>>>(k,v,n,card); CK(cudaDeviceSynchronize());
+  gen<<<132*8,256>>>(k,v,n,card); CK(cudaDeviceSynchronize());
   const char* names[]={"stream-only","SoA 2xRED","AoS16 2xRED","AoS16 1xRED","AoS16 paired","slot32 probe+2RED","slot32 probe+paired","SoA 2xATOM(ret)","slot32 probe only"};
   for(int gm=4; gm<=16; gm*=2){
-    int grid=148*gm;
+    int grid=132*gm;
     float ms[9];
     ms[0]=run<0>(k,v,n,t0,t1,tbytes,slots-1,sink,grid); ms[1]=run<1>(k,v,n,t0,t1,tbytes,slots-1,sink,grid);
     ms[2]=run<2>(k,v,n,t0,t1,tbytes,slots-1,sink,grid); ms[3]=run<3>(k,v,n,t0,t1,tbytes,slots-1,sink,grid);

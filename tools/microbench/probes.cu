@@ -1,5 +1,5 @@
 // Microbenchmark 2: cost of the hash-probe load flavour and of the table size (L2 residency across the two dies).
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o probes probes.cu
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o probes probes.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>
@@ -34,7 +34,7 @@ __global__ void __launch_bounds__(256) k(const int64_t* __restrict__ keys, size_
 }
 template<int F,int R> float run(const int64_t* keys,size_t n,unsigned long long* t,uint64_t mask,unsigned long long* sink,unsigned long long* t2=nullptr){
   cudaEvent_t a,b; CK(cudaEventCreate(&a)); CK(cudaEventCreate(&b)); float best=1e9;
-  for(int it=0;it<3;it++){ CK(cudaEventRecord(a)); k<F,R><<<148*8,256>>>(keys,n,t,mask,sink,t2); CK(cudaEventRecord(b)); CK(cudaEventSynchronize(b)); CK(cudaGetLastError()); float ms; CK(cudaEventElapsedTime(&ms,a,b)); if(it>0&&ms<best)best=ms; }
+  for(int it=0;it<3;it++){ CK(cudaEventRecord(a)); k<F,R><<<132*8,256>>>(keys,n,t,mask,sink,t2); CK(cudaEventRecord(b)); CK(cudaEventSynchronize(b)); CK(cudaGetLastError()); float ms; CK(cudaEventElapsedTime(&ms,a,b)); if(it>0&&ms<best)best=ms; }
   return best;
 }
 int main(){
@@ -42,7 +42,7 @@ int main(){
   const char* names[]={"ld.relaxed.gpu","ld.global.cg","ld.global.nc","ld.global","ld.volatile"};
   for(int lg=18; lg<=23; lg++){
     size_t slots=(size_t)1<<lg; unsigned long long* t; CK(cudaMalloc(&t,slots*32));
-    fill<<<148*8,256>>>(t,slots); gen<<<148*8,256>>>(keys,n,slots); CK(cudaDeviceSynchronize());
+    fill<<<132*8,256>>>(t,slots); gen<<<132*8,256>>>(keys,n,slots); CK(cudaDeviceSynchronize());
     float ms[5][2];
     ms[0][0]=run<0,0>(keys,n,t,slots-1,sink); ms[0][1]=run<0,1>(keys,n,t,slots-1,sink);
     ms[1][0]=run<1,0>(keys,n,t,slots-1,sink); ms[1][1]=run<1,1>(keys,n,t,slots-1,sink);

@@ -7,7 +7,7 @@
 //           slice of the dense {sum, count} table with plain stores (a key lives in exactly one bucket)
 //
 // The comparison points are the shipped forms: one RED sector per row into the L2-resident table ("direct") and the stream alone.
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o radix_prepass radix_prepass.cu
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o radix_prepass radix_prepass.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>
@@ -23,8 +23,8 @@ __global__ void gen(int64_t* k, int64_t* v, size_t n, uint64_t card){
   for(;i<n;i+=st){ uint64_t h=mix(i*0x9E3779B97F4A7C15ULL+12345); k[i]=(int64_t)(h%card); v[i]=(int64_t)(mix(h)%2000000)-1000000; }
 }
 __device__ __forceinline__ void red64(unsigned long long* p, unsigned long long v){ asm volatile("red.global.add.u64 [%0], %1;"::"l"(p),"l"(v):"memory"); }
-__device__ __forceinline__ void ld256(const int64_t* p, int64_t (&r)[4]){
-  asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v4.s64 {%0,%1,%2,%3}, [%4];":"=l"(r[0]),"=l"(r[1]),"=l"(r[2]),"=l"(r[3]):"l"(p));
+__device__ __forceinline__ void ld256(const int64_t* p, int64_t (&r)[4]){   // two 128-bit loads: the widest on sm_90
+  asm volatile("{.reg .b64 pol; createpolicy.fractional.L2::evict_first.b64 pol, 1.0;\n\tld.global.nc.L1::no_allocate.L2::cache_hint.v2.s64 {%0,%1}, [%4], pol;\n\tld.global.nc.L1::no_allocate.L2::cache_hint.v2.s64 {%2,%3}, [%4+16], pol;}":"=l"(r[0]),"=l"(r[1]),"=l"(r[2]),"=l"(r[3]):"l"(p));
 }
 
 // ---------------------------------------------------------------- the shipped form: one paired RED per row
@@ -112,7 +112,7 @@ __global__ void __launch_bounds__(THREADS) partition_kernel(const int64_t* __res
 }
 
 // ---------------------------------------------------------------- pass 2: one CTA per bucket, shared-memory table
-// 64-bit shared-memory atomicAdd is a CAS loop on sm_100 (SASS ATOMS.CAST.SPIN.64); 32-bit ones are native (ATOMS.ADD / ATOMS.POPC.INC). MODE:
+// 64-bit shared-memory atomicAdd is a CAS loop on sm_90a (SASS ATOMS.CAST.SPIN.64); 32-bit ones are native (ATOMS.ADD / ATOMS.POPC.INC). MODE:
 //   0  sum: 64-bit CAS loop, count: 32-bit            1  sum: 32-bit add with the old value returned + a carry add into a high word when it wraps, count: 32-bit
 //   2  ONE 64-bit CAS loop on {count : 24 | sum : 40} 3  like 1 without the carry (an upper bound: exact only while a key's sum stays below 2^32)
 template<int MODE>
@@ -185,7 +185,7 @@ int main(int argc, char** argv) {
   int64_t *k, *v; CK(cudaMalloc(&k, n * 8)); CK(cudaMalloc(&v, n * 8)); gen<<<sms * 8, 256>>>(k, v, n, card); CK(cudaDeviceSynchronize());
   unsigned long long *tab, *tab_ref; CK(cudaMalloc(&tab, card * 16)); CK(cudaMalloc(&tab_ref, card * 16));
   cudaStream_t s; CK(cudaStreamCreate(&s));
-  const double hbm = 6569.0;
+  const double hbm = 3350.0;                                            // GB/s: H100 SXM data-sheet HBM3 bandwidth
   // reference result + the shipped form's time
   float ms_direct = time_ms(s, 5, [&]{ direct_kernel<<<sms * 4, 512, 0, s>>>(k, v, n, tab_ref); }, [&]{ CK(cudaMemsetAsync(tab_ref, 0, card * 16, s)); });
   printf("%-58s %7.3f ms  %6.1f Grows/s  frac(16 B/row) %.3f\n", "direct: paired RED into the L2-resident table", ms_direct, n / ms_direct / 1e6, 16.0 * n / ms_direct / 1e6 / hbm);
