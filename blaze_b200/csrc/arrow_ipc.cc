@@ -111,8 +111,9 @@ DType parse_field_type(const Table& field) {
       if (unit != 2) throw PlanError(B200Q_ERR_UNSUPPORTED, "literal: only timestamp[us]");
       d.id = T_TIMESTAMP_US; return d;
     }
-    case TY_Utf8: case TY_Binary:
-      throw PlanError(B200Q_ERR_UNSUPPORTED, "literal: string/binary literals are not on the hot path");
+    case TY_Utf8: d.id = T_UTF8; return d;
+    case TY_Binary:
+      throw PlanError(B200Q_ERR_UNSUPPORTED, "literal: binary literals are not on the hot path");
     default:
       throw PlanError(B200Q_ERR_UNSUPPORTED, "literal: unsupported arrow type tag " + std::to_string(tt));
   }
@@ -159,7 +160,13 @@ ExprP decode_ipc_literal(const uint8_t* bytes, size_t n) {
       bool valid = true;
       if (null_count > 0) valid = vlen > 0 ? (body[voff] & 1) != 0 : false;
       e->lit_null = !valid;
-      if (valid) {
+      if (valid && e->type.id == T_UTF8) {         // buffers: validity, int32 offsets (row 0: [o0, o1)), data
+        int64_t xoff, xlen; buf_at(2, xoff, xlen);
+        if (dlen < 8) throw PlanError(B200Q_ERR_INVALID_PLAN, "literal: Utf8 offsets buffer too short");
+        int32_t o0, o1; memcpy(&o0, body + doff, 4); memcpy(&o1, body + doff + 4, 4);
+        if (o0 < 0 || o1 < o0 || (int64_t)o1 > xlen) throw PlanError(B200Q_ERR_INVALID_PLAN, "literal: Utf8 offsets out of the data buffer");
+        e->lit_str.assign((const char*)body + xoff + o0, (size_t)(o1 - o0));
+      } else if (valid) {
         const uint8_t* d = body + doff;
         auto need = [&](int64_t w) { if (dlen < w) throw PlanError(B200Q_ERR_INVALID_PLAN, "literal: value buffer too short"); };
         switch (e->type.id) {

@@ -24,14 +24,14 @@ static std::string format_of(const DType& t) {
     case T_BOOL: return "b"; case T_INT8: return "c"; case T_INT16: return "s"; case T_INT32: return "i"; case T_INT64: return "l";
     case T_FLOAT32: return "f"; case T_FLOAT64: return "g"; case T_DATE32: return "tdD"; case T_TIMESTAMP_US: return "tsu:";
     case T_DECIMAL128: return "d:" + std::to_string(t.precision) + "," + std::to_string(t.scale);
-    case T_BINARY: return "z"; default: return "n";
+    case T_BINARY: return "z"; case T_UTF8: return "u"; default: return "n";
   }
 }
 DType type_of_format(const char* f) {
   DType d; std::string s(f ? f : "");
   if (s == "b") d.id = T_BOOL; else if (s == "c") d.id = T_INT8; else if (s == "s") d.id = T_INT16; else if (s == "i") d.id = T_INT32;
   else if (s == "l") d.id = T_INT64; else if (s == "f") d.id = T_FLOAT32; else if (s == "g") d.id = T_FLOAT64; else if (s == "tdD") d.id = T_DATE32;
-  else if (s.rfind("tsu:", 0) == 0) d.id = T_TIMESTAMP_US; else if (s == "z") d.id = T_BINARY; else if (s == "n") d.id = T_NULL;
+  else if (s.rfind("tsu:", 0) == 0) d.id = T_TIMESTAMP_US; else if (s == "z") d.id = T_BINARY; else if (s == "u") d.id = T_UTF8; else if (s == "n") d.id = T_NULL;
   else if (s.rfind("d:", 0) == 0) {
     int p = 0, sc = 0, bw = 128; if (sscanf(s.c_str(), "d:%d,%d,%d", &p, &sc, &bw) < 2 || bw != 128) throw PlanError(B200Q_ERR_UNSUPPORTED, "unsupported decimal format " + s);
     d.id = T_DECIMAL128; d.precision = (uint8_t)p; d.scale = (int8_t)sc;
@@ -158,6 +158,9 @@ static void build_pipeline(b200q_op* op) {
   for (PlanNode* n = op->plan.get(); n; n = n->input.get()) chain.push_back(n);
   std::reverse(chain.begin(), chain.end());
   if (chain.empty() || chain[0]->kind != N_LEAF) throw PlanError(B200Q_ERR_INVALID_PLAN, "plan has no leaf");
+  if (chain[0]->leaf_kind == "ParquetScan")
+    for (auto& f : chain[0]->schema.fields)
+      if (f.type.is_varlen()) throw PlanError(B200Q_ERR_UNSUPPORTED, "ParquetScanExec: column " + f.name + " is " + f.type.str() + "; BYTE_ARRAY decode is not on the GPU path");
   op->in_schema = chain[0]->schema;
   SchemaDef stage_in = chain[0]->schema;
   std::vector<ExprP> cur_cols = identity_cols(stage_in), filters;
@@ -249,11 +252,11 @@ static void validate_host_batch(b200q_op* op, const ArrowArray* batch) {
     // the import paths dereference buffers[1] (and buffers[2] of Binary columns): a malformed / foreign batch must not crash the host process
     const DType& t = op->in_schema.fields[(size_t)i].type;
     if (t.id == T_NULL || batch->length == 0) continue;
-    const int need = t.id == T_BINARY ? 3 : 2;
+    const int need = t.is_varlen() ? 3 : 2;
     if (c->n_buffers < need || !c->buffers) throw ExecError(B200Q_ERR_INVALID_ARG, "push: column " + std::to_string(i) + " has " + std::to_string(c->n_buffers) + " buffers, its type needs " + std::to_string(need));
-    if (!c->buffers[1]) throw ExecError(B200Q_ERR_INVALID_ARG, "push: column " + std::to_string(i) + " has a null " + (t.id == T_BINARY ? "offsets" : "values") + " buffer");
-    if (t.id == T_BINARY && !c->buffers[2] && ((const int32_t*)c->buffers[1])[c->offset + batch->offset + batch->length] != ((const int32_t*)c->buffers[1])[c->offset + batch->offset])
-      throw ExecError(B200Q_ERR_INVALID_ARG, "push: binary column " + std::to_string(i) + " has a null data buffer");
+    if (!c->buffers[1]) throw ExecError(B200Q_ERR_INVALID_ARG, "push: column " + std::to_string(i) + " has a null " + (t.is_varlen() ? "offsets" : "values") + " buffer");
+    if (t.is_varlen() && !c->buffers[2] && ((const int32_t*)c->buffers[1])[c->offset + batch->offset + batch->length] != ((const int32_t*)c->buffers[1])[c->offset + batch->offset])
+      throw ExecError(B200Q_ERR_INVALID_ARG, "push: " + t.str() + " column " + std::to_string(i) + " has a null data buffer");
   }
 }
 
@@ -287,17 +290,23 @@ static DevBatch import_direct(b200q_op* op, const ArrowArray* batch, const std::
       dc.validity = DevMem::alloc(nb + 4, cx.stream);
       B200Q_CUDA(cudaMemcpyAsync(dc.validity->ptr, validity + a0 / 8, nb, cudaMemcpyHostToDevice, cx.stream)); cx.m.h2d_bytes += (int64_t)nb;
     }
-    if (dc.type.id == T_BINARY) {
-      if (c->n_buffers < 3) throw ExecError(B200Q_ERR_INVALID_ARG, "binary column needs 3 buffers");
+    if (dc.type.is_varlen()) {
+      if (c->n_buffers < 3) throw ExecError(B200Q_ERR_INVALID_ARG, dc.type.str() + " column needs 3 buffers");
       const int32_t* offs = (const int32_t*)c->buffers[1]; const uint8_t* data = (const uint8_t*)c->buffers[2];
       const int32_t first = offs[a0], end = offs[off + len];
       dc.offsets = DevMem::alloc((size_t)(cnt + 1) * 4, cx.stream);
-      B200Q_CUDA(cudaMemcpyAsync(dc.offsets->ptr, offs + a0, (size_t)(cnt + 1) * 4, cudaMemcpyHostToDevice, cx.stream));
-      DevMemP d = DevMem::alloc((size_t)(end - first), cx.stream);
-      if (end > first) B200Q_CUDA(cudaMemcpyAsync(d->ptr, data + first, (size_t)(end - first), cudaMemcpyHostToDevice, cx.stream));
+      // only [first, end) of the data is copied: the device offsets are rebased to start at 0, so every imported column indexes its
+      // own allocation (columns may then be shared with the output and exported as they are)
+      if (first == 0) B200Q_CUDA(cudaMemcpyAsync(dc.offsets->ptr, offs + a0, (size_t)(cnt + 1) * 4, cudaMemcpyHostToDevice, cx.stream));
+      else {
+        std::vector<int32_t> rebased(offs + a0, offs + a0 + cnt + 1);
+        for (auto& o : rebased) o -= first;
+        // a pageable source: the call returns once `rebased` has been staged, so it may go out of scope
+        B200Q_CUDA(cudaMemcpyAsync(dc.offsets->ptr, rebased.data(), (size_t)(cnt + 1) * 4, cudaMemcpyHostToDevice, cx.stream));
+      }
+      dc.values = DevMem::alloc((size_t)(end - first), cx.stream);
+      if (end > first) B200Q_CUDA(cudaMemcpyAsync(dc.values->ptr, data + first, (size_t)(end - first), cudaMemcpyHostToDevice, cx.stream));
       cx.m.h2d_bytes += (int64_t)(cnt + 1) * 4 + (end - first);
-      // kernels address data + offsets[i] with absolute offsets: bias the base pointer
-      dc.values = DevMem::borrow((const uint8_t*)d->ptr - first, (size_t)end, d);
     } else if (dc.type.id == T_BOOL) {
       const size_t nb = (size_t)((cnt + 7) / 8);
       dc.values = DevMem::alloc(nb + 4, cx.stream);
@@ -320,7 +329,7 @@ static void staging_init(b200q_op* op, const std::vector<int>& used) {
     B200Q_CUDA(cudaEventCreateWithFlags(&st.ev, cudaEventDisableTiming));
     for (int ci : used) {
       const DType& t = op->in_schema.fields[ci].type; StagingSet::Col& c = st.cols[ci];
-      if (t.id == T_BINARY) {
+      if (t.is_varlen()) {
         B200Q_CUDA(cudaMallocHost((void**)&c.offsets, (size_t)(cap + 1) * 4)); c.offsets[0] = 0;
         c.data_cap = (size_t)cap * 32; B200Q_CUDA(cudaMallocHost((void**)&c.data, c.data_cap));
       } else if (t.id == T_BOOL) { c.values_cap = (size_t)(cap + 7) / 8 + 8; B200Q_CUDA(cudaMallocHost(&c.values, c.values_cap)); memset(c.values, 0, c.values_cap); }
@@ -351,7 +360,7 @@ static void staging_flush(b200q_op* op) {
     StagingSet::Col& c = st.cols[ci]; DevColumn& dc = db.cols[ci];
     const int64_t n = st.rows;
     if (c.validity && c.any_null) { const size_t nb = (size_t)(n + 7) / 8; dc.validity = DevMem::alloc(nb + 4, cx.stream); B200Q_CUDA(cudaMemcpyAsync(dc.validity->ptr, c.validity, nb, cudaMemcpyHostToDevice, cx.stream)); cx.m.h2d_bytes += (int64_t)nb; }
-    if (dc.type.id == T_BINARY) {
+    if (dc.type.is_varlen()) {
       dc.offsets = DevMem::alloc((size_t)(n + 1) * 4, cx.stream); B200Q_CUDA(cudaMemcpyAsync(dc.offsets->ptr, c.offsets, (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, cx.stream));
       dc.values = DevMem::alloc(c.data_len, cx.stream); if (c.data_len) B200Q_CUDA(cudaMemcpyAsync(dc.values->ptr, c.data, c.data_len, cudaMemcpyHostToDevice, cx.stream));
       cx.m.h2d_bytes += (int64_t)(n + 1) * 4 + (int64_t)c.data_len;
@@ -383,7 +392,7 @@ static void staging_append(b200q_op* op, const ArrowArray* batch) {
       const int64_t off = c->offset + batch->offset + done;
       const uint8_t* validity = c->n_buffers > 0 ? (const uint8_t*)c->buffers[0] : nullptr;
       if (sc.validity) { if (validity && c->null_count != 0) { copy_bits(sc.validity, st.rows, validity, off, take); sc.any_null = true; } else set_bits(sc.validity, st.rows, take); }
-      if (t.id == T_BINARY) {
+      if (t.is_varlen()) {
         const int32_t* offs = (const int32_t*)c->buffers[1]; const uint8_t* data = (const uint8_t*)c->buffers[2];
         const size_t nbytes = (size_t)(offs[off + take] - offs[off]);
         if (sc.data_len + nbytes > sc.data_cap) {
@@ -423,11 +432,13 @@ static HostBatch to_host(b200q_op* op, DevBatch& db) {
     if (dc.offset != 0) throw ExecError(B200Q_ERR_EXECUTION, "internal: output column with non-zero offset");
     auto d2h = [&](const void* src, size_t bytes) { void* p = hb.block->alloc(bytes + 8); if (bytes) B200Q_CUDA(cudaMemcpyAsync(p, src, bytes, cudaMemcpyDeviceToHost, cx.stream)); cx.m.d2h_bytes += (int64_t)bytes; return p; };
     if (dc.validity) hc.validity = d2h(dc.validity->ptr, (size_t)(n + 7) / 8);
-    if (dc.type.id == T_BINARY) {
+    if (dc.type.is_varlen()) {
       hc.offsets = d2h(dc.offsets->ptr, (size_t)(n + 1) * 4);
       B200Q_CUDA(cudaStreamSynchronize(cx.stream));
-      const int32_t total = ((int32_t*)hc.offsets)[n];
-      hc.values = d2h(dc.values->ptr, (size_t)total);
+      int32_t* ho = (int32_t*)hc.offsets;
+      const int32_t first = ho[0];                          // only the bytes the rows reference; the host copy starts at 0
+      hc.values = d2h((const uint8_t*)dc.values->ptr + first, (size_t)(ho[n] - first));
+      if (first) for (int64_t i = 0; i <= n; i++) ho[i] -= first;
     } else if (dc.type.id == T_BOOL) hc.values = d2h(dc.values->ptr, (size_t)(n + 7) / 8);
     else if (dc.type.id != T_NULL) hc.values = d2h(dc.values->ptr, (size_t)n * dc.type.byte_width());
     hb.cols.push_back(hc);
@@ -466,7 +477,7 @@ static void export_host_slice(const HostBatch& hb, int64_t off, int64_t len, Arr
     c.length = len; c.offset = off;
     c.null_count = hc.validity ? count_nulls((const uint8_t*)hc.validity, off, len) : 0;
     if (hc.type.id == T_NULL) { c.null_count = len; c.n_buffers = 0; }
-    else if (hc.type.id == T_BINARY) { cp->buffers = {hc.validity, hc.offsets, hc.values}; c.n_buffers = 3; }
+    else if (hc.type.is_varlen()) { cp->buffers = {hc.validity, hc.offsets, hc.values}; c.n_buffers = 3; }
     else { cp->buffers = {hc.validity, hc.values}; c.n_buffers = 2; }
     c.buffers = cp->buffers.data(); c.release = release_array; c.private_data = cp;
     top->child_ptrs[i] = &c;
@@ -490,7 +501,7 @@ void export_device(DevBatch& db, int device, ArrowDeviceArray* out) {
     if (dc.values) cp->dev.push_back(dc.values);
     if (dc.offsets) cp->dev.push_back(dc.offsets);
     if (dc.type.id == T_NULL) { c.n_buffers = 0; c.null_count = db.num_rows; }
-    else if (dc.type.id == T_BINARY) { cp->buffers = {v, dc.offsets->ptr, dc.values->ptr}; c.n_buffers = 3; }
+    else if (dc.type.is_varlen()) { cp->buffers = {v, dc.offsets->ptr, dc.values->ptr}; c.n_buffers = 3; }
     else { cp->buffers = {v, dc.values ? dc.values->ptr : nullptr}; c.n_buffers = 2; }
     c.buffers = cp->buffers.data(); c.release = release_array; c.private_data = cp;
     top->child_ptrs[i] = &c;
@@ -638,7 +649,7 @@ b200q_status b200q_op_push_device(b200q_op* op, struct ArrowDeviceArray* dbatch)
       dc.type = op->in_schema.fields[i].type; dc.offset = c->offset + batch->offset;
       const size_t huge = (size_t)1 << 60;
       if (c->n_buffers > 0 && c->buffers[0] && c->null_count != 0) dc.validity = DevMem::borrow(c->buffers[0], huge, nullptr);
-      if (dc.type.id == T_BINARY) { dc.offsets = DevMem::borrow(c->buffers[1], huge, nullptr); dc.values = DevMem::borrow(c->buffers[2], huge, nullptr); }
+      if (dc.type.is_varlen()) { dc.offsets = DevMem::borrow(c->buffers[1], huge, nullptr); dc.values = DevMem::borrow(c->buffers[2], huge, nullptr); }
       else if (c->n_buffers > 1 && c->buffers[1]) dc.values = DevMem::borrow(c->buffers[1], huge, nullptr);
     }
     // queued BEFORE the stages run: if a stage throws, the array is still released (poll_pending) and the event destroyed;
@@ -830,6 +841,7 @@ b200q_status b200q_murmur3_partition(const struct ArrowSchema* key_schema, const
     ColTable ct{}; uint8_t phys[VM_MAX_COLS];
     for (int64_t i = 0; i < a.n_children; i++) {
       const DType t = type_of_format(key_schema->children[i]->format);
+      if (t.is_varlen()) throw ExecError(B200Q_ERR_UNSUPPORTED, "murmur3 partition ids over a " + t.str() + " key are not on the GPU path");
       const ArrowArray* c = a.children[i];
       DevColumn dc; dc.type = t; dc.offset = c->offset + a.offset;
       phys[i] = phys_of(t);

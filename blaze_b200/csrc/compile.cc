@@ -3,6 +3,7 @@
 // (project_exec.rs:143-149); on the GPU the whole Filter/Project chain below an Agg fuses the same
 // way, so filtered rows never round-trip through HBM.
 #include <cmath>
+#include <cstddef>
 #include <cstring>
 
 #include "../../include/blaze_b200.h"
@@ -18,7 +19,7 @@ PhysKind phys_of(const DType& t) {
   switch (t.id) {
     case T_BOOL: return PH_BOOL; case T_INT8: return PH_I8; case T_INT16: return PH_I16;
     case T_INT32: case T_DATE32: return PH_I32; case T_INT64: case T_TIMESTAMP_US: return PH_I64;
-    case T_FLOAT32: return PH_F32; case T_FLOAT64: return PH_F64; case T_DECIMAL128: return PH_DEC128;
+    case T_FLOAT32: return PH_F32; case T_FLOAT64: return PH_F64; case T_DECIMAL128: return PH_DEC128; case T_UTF8: return PH_STR;
     default: throw PlanError(B200Q_ERR_UNSUPPORTED, "column type " + t.str() + " cannot be evaluated on the device");
   }
 }
@@ -64,7 +65,20 @@ struct Compiler {
     return (int)out.used_cols.size() - 1;
   }
 
-  static int slots(const DType& t) { return t.is_decimal() ? 2 : 1; }
+  static int slots(const DType& t) { return t.is_decimal() || t.id == T_UTF8 ? 2 : 1; }
+
+  // a Utf8 constant: its bytes go to the program's string pool, the pool gets {offset, length} (relocated to a device address at upload)
+  uint32_t str_const(const std::string& v) {
+    if (p().n_str + v.size() > (size_t)VM_MAX_STR_POOL)
+      throw PlanError(B200Q_ERR_UNSUPPORTED, "string literals of one fused pipeline exceed the " + std::to_string(VM_MAX_STR_POOL) + "-byte literal pool of the device evaluator");
+    const uint32_t off = p().n_str;
+    if (!v.empty()) memcpy(p().str_pool + off, v.data(), v.size());
+    p().n_str += (uint32_t)v.size();
+    out.has_strings = true;
+    const uint32_t at = pool({off, (uint64_t)v.size()});
+    out.str_relocs.push_back(at);
+    return at;
+  }
 
   void push_null(int nslots) { emit(VM_LOAD_LIT, (uint8_t)(1 | (nslots == 2 ? 2 : 0)), 0, pool({0, 0})); push(nslots); }
 
@@ -74,10 +88,12 @@ struct Compiler {
     switch (e->kind) {
       case E_COLUMN: {
         PhysKind ph = phys_of(e->type);
+        if (ph == PH_STR) { out.has_strings = true; emit(VM_LOAD_STR, 0, (uint16_t)col_slot(e->col_index)); push(2); return 2; }
         emit(VM_LOAD_COL, ph, (uint16_t)col_slot(e->col_index)); push(slots(e->type)); return slots(e->type);
       }
       case E_LITERAL: {
         int n = slots(e->type);
+        if (e->type.id == T_UTF8) { emit(VM_LOAD_LIT, (uint8_t)((e->lit_null ? 1 : 0) | 2), 0, str_const(e->lit_str)); push(2); return 2; }
         emit(VM_LOAD_LIT, (uint8_t)((e->lit_null ? 1 : 0) | (n == 2 ? 2 : 0)), 0, pool({e->lit_lo, e->lit_hi})); push(n); return n;
       }
       case E_BINARY: case E_SC_AND: case E_SC_OR: return binary(e);
@@ -95,6 +111,12 @@ struct Compiler {
       case E_CASE: return case_(e);
       case E_IN_LIST: return in_list(e);
       case E_SCALAR_FN: return scalar_fn(e);
+      case E_STR_MATCH: {
+        expr(e->children[0]);
+        emit(VM_LOAD_LIT, 2, 0, str_const(e->lit_str)); push(2);
+        static const VmOp ops[] = {VM_STARTS_WITH, VM_ENDS_WITH, VM_CONTAINS};
+        emit(ops[e->str_match]); pop(4); push(1); return 1;
+      }
     }
     throw PlanError(B200Q_ERR_UNSUPPORTED, "unsupported expression kind");
   }
@@ -107,7 +129,7 @@ struct Compiler {
     if (op >= OP_EQ && op <= OP_GE) {
       int n = expr(l); expr(r);
       uint8_t c = (uint8_t)(op - OP_EQ);   // OP_EQ..OP_GE map to CMP_EQ,NE,LT,LE,GT,GE in the same order
-      if (t.is_decimal()) emit(VM_CMP_DEC, c); else if (t.is_float()) emit(VM_CMP_F, c); else emit(VM_CMP_I, c);
+      if (t.id == T_UTF8) emit(VM_CMP_STR, c); else if (t.is_decimal()) emit(VM_CMP_DEC, c); else if (t.is_float()) emit(VM_CMP_F, c); else emit(VM_CMP_I, c);
       pop(2 * n); push(1); return 1;
     }
     if (op >= OP_BIT_AND) { expr(l); expr(r); emit(op == OP_BIT_AND ? VM_BIT_AND : op == OP_BIT_OR ? VM_BIT_OR : VM_BIT_XOR); pop(2); push(1); return 1; }
@@ -132,6 +154,7 @@ struct Compiler {
     if (from.id == T_NULL) { push_null(slots(to)); return slots(to); }       // cast of an untyped NULL
     int n = expr(e->children[0]);
     if (from == to) return n;                                                 // commons cast.rs:41
+    if (from.id == T_UTF8 && to.is_integer() && e->kind == E_TRY_CAST) { emit(VM_CAST_STR_I, (uint8_t)to.int_bits()); pop(2); push(1); return 1; }
     auto ii = [](const DType& t) { return t.is_integer() || t.id == T_DATE32 || t.id == T_TIMESTAMP_US; };
     i128 lim = to.is_decimal() ? pow10_i128(to.precision) : 0;
     if (ii(from) && ii(to)) { if (to.int_bits() < from.int_bits()) emit(VM_CAST_I_I, (uint8_t)to.int_bits()); return 1; }
@@ -168,6 +191,7 @@ struct Compiler {
     //   result = SELECT(c1, t1, SELECT(c2, t2, ... else))   -- build from the last WHEN backwards
     size_t i0 = e->case_has_base ? 1 : 0;
     size_t nwt = (e->children.size() - i0 - (e->case_has_else ? 1 : 0)) / 2;
+    if (e->type.id == T_UTF8 || (e->case_has_base && e->children[0]->type.id == T_UTF8)) throw PlanError(B200Q_ERR_UNSUPPORTED, "CASE over strings is not on the hot path");
     int n = slots(e->type);
     // emit conditions and THENs in order, then ELSE, then fold with SELECTs (stack: c1 t1 c2 t2 ... else)
     for (size_t k = 0; k < nwt; k++) {
@@ -187,6 +211,7 @@ struct Compiler {
 
   int in_list(const ExprP& e) {
     const ExprP& x = e->children[0];
+    if (x->type.id == T_UTF8) return in_list_str(e);
     int kind = x->type.is_decimal() ? 2 : x->type.is_float() ? 1 : 0;
     bool has_null = false; std::vector<uint64_t> items;
     for (size_t i = 1; i < e->children.size(); i++) {
@@ -204,6 +229,20 @@ struct Compiler {
     for (auto v : items) p().pool[p().n_pool++] = v;
     uint16_t cnt = (uint16_t)(kind == 2 ? items.size() / 2 : items.size());
     emit(VM_IN_LIST, (uint8_t)(kind | (e->negated ? 4 : 0) | (has_null ? 8 : 0)), cnt, at); pop(n); push(1); return 1;
+  }
+
+  int in_list_str(const ExprP& e) {
+    bool has_null = false; std::vector<const std::string*> items;
+    for (size_t i = 1; i < e->children.size(); i++) {
+      ExprP it = e->children[i];
+      if ((it->kind == E_TRY_CAST || it->kind == E_CAST) && it->children[0]->kind == E_LITERAL && it->children[0]->type.id == T_NULL) it = it->children[0];   // TryCast(NULL)
+      if (it->kind != E_LITERAL || !(it->type.id == T_UTF8 || it->type.id == T_NULL)) throw PlanError(B200Q_ERR_UNSUPPORTED, "IN list items must be literals on the hot path");
+      if (it->lit_null || it->type.id == T_NULL) has_null = true; else items.push_back(&it->lit_str);
+    }
+    int n = expr(e->children[0]);
+    uint32_t at = p().n_pool;
+    for (auto* s : items) str_const(*s);                     // consecutive {ptr, len} pairs
+    emit(VM_IN_LIST, (uint8_t)(3 | (e->negated ? 4 : 0) | (has_null ? 8 : 0)), (uint16_t)items.size(), at); pop(n); push(1); return 1;
   }
 
   // constant-fold Literal / TryCast(Literal) to `want` (only the conversions IN lists need)
@@ -260,7 +299,7 @@ struct Compiler {
 
 }  // namespace
 
-CompiledProgram compile_program(const std::vector<ExprP>& filters, const std::vector<ExprP>& outs, bool with_compact) {
+CompiledProgram compile_program(const std::vector<ExprP>& filters, const std::vector<ExprP>& outs, bool with_compact, int sel_out) {
   Compiler c;
   memset(&c.out.prog, 0, sizeof(VmProgram));
   for (auto& f : filters) {
@@ -269,15 +308,23 @@ CompiledProgram compile_program(const std::vector<ExprP>& filters, const std::ve
   }
   c.out.prog.n_filters = (uint32_t)filters.size();
   if (with_compact) c.emit(VM_COMPACT);
-  if (outs.size() > VM_MAX_OUT) throw PlanError(B200Q_ERR_UNSUPPORTED, "too many outputs for one fused pipeline");
+  if (outs.size() + (sel_out >= 0 ? 1 : 0) > VM_MAX_OUT) throw PlanError(B200Q_ERR_UNSUPPORTED, "too many outputs for one fused pipeline");
   for (size_t i = 0; i < outs.size(); i++) {
     const ExprP& e = outs[i];
     int n = c.expr(e);
     c.emit(VM_OUT, (uint8_t)phys_of(e->type), (uint16_t)i); c.pop(n);
     c.out.outs.push_back(OutDesc{e->type, e->nullable, n});
   }
+  if (sel_out >= 0) c.emit(VM_OUT_SEL, 0, (uint16_t)sel_out);
   c.emit(VM_END);
   return c.out;
+}
+
+VmProgram relocated_program(const CompiledProgram& cp, const void* device_copy) {
+  VmProgram p = cp.prog;
+  const uint64_t base = (uint64_t)(uintptr_t)device_copy + offsetof(VmProgram, str_pool);
+  for (uint32_t i : cp.str_relocs) p.pool[i] += base;
+  return p;
 }
 
 }  // namespace b200q

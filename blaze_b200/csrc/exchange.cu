@@ -237,7 +237,7 @@ b200q_status b200q_exchange_shuffle(b200q_exchange* ex, const struct ArrowSchema
     ColTable kt{}; uint8_t kphys[VM_MAX_COLS];
     for (int i = 0; i < ncols; i++) {
       types[i] = type_of_format(schema->children[i]->format);
-      if (types[i].id == T_BINARY || types[i].id == T_BOOL || types[i].id == T_NULL) throw ExecError(B200Q_ERR_UNSUPPORTED, "exchange: only fixed-width columns travel GPU-to-GPU (use partial_state_columnar = 1)");
+      if (types[i].is_varlen() || types[i].id == T_BOOL || types[i].id == T_NULL) throw ExecError(B200Q_ERR_UNSUPPORTED, "exchange: only fixed-width columns travel GPU-to-GPU (use partial_state_columnar = 1)");
       const ArrowArray* c = a.children[i];
       nullable[i] = c->n_buffers > 0 && c->buffers[0] && c->null_count != 0;
       if (i < n_key_cols) {

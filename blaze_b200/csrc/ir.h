@@ -11,7 +11,7 @@ namespace b200q {
 
 // must match blaze_b200/types.py
 enum TypeId : uint8_t { T_BOOL = 0, T_INT8, T_INT16, T_INT32, T_INT64, T_FLOAT32, T_FLOAT64, T_DATE32,
-                        T_TIMESTAMP_US, T_DECIMAL128, T_BINARY, T_NULL };
+                        T_TIMESTAMP_US, T_DECIMAL128, T_BINARY, T_NULL, T_UTF8 };
 
 struct DType {
   TypeId id = T_NULL;
@@ -22,6 +22,8 @@ struct DType {
   bool is_integer() const { return id >= T_INT8 && id <= T_INT64; }
   bool is_float() const { return id == T_FLOAT32 || id == T_FLOAT64; }
   bool is_decimal() const { return id == T_DECIMAL128; }
+  // offsets + data buffers (Arrow Utf8 / Binary): imported, exported and carried through one code path
+  bool is_varlen() const { return id == T_UTF8 || id == T_BINARY; }
   // ints, bool, date32, timestamp all travel as sign-extended i64 on the device
   bool is_intlike() const { return is_integer() || id == T_BOOL || id == T_DATE32 || id == T_TIMESTAMP_US; }
   int byte_width() const {
@@ -53,7 +55,9 @@ struct PlanError : std::runtime_error {
 };
 
 enum ExprKind : uint8_t { E_COLUMN, E_LITERAL, E_BINARY, E_IS_NULL, E_IS_NOT_NULL, E_NOT, E_NEGATIVE, E_CAST,
-                          E_TRY_CAST, E_CASE, E_IN_LIST, E_SC_AND, E_SC_OR, E_SCALAR_FN };
+                          E_TRY_CAST, E_CASE, E_IN_LIST, E_SC_AND, E_SC_OR, E_SCALAR_FN, E_STR_MATCH };
+// E_STR_MATCH: StringStartsWith / EndsWith / Contains ExprNode (auron.proto:339-352); pattern in lit_str
+enum StrMatch : uint8_t { SM_STARTS_WITH = 0, SM_ENDS_WITH, SM_CONTAINS };
 enum BinOp : uint8_t { OP_AND, OP_OR, OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE, OP_PLUS, OP_MINUS, OP_MUL, OP_DIV,
                        OP_MOD, OP_BIT_AND, OP_BIT_OR, OP_BIT_XOR };
 
@@ -70,10 +74,13 @@ struct Expr {
   // E_LITERAL: value bits (decimal: lo/hi of the i128; float: IEEE bits of f64 (f32 widened); int: sign-extended)
   bool lit_null = false;
   uint64_t lit_lo = 0, lit_hi = 0;
+  std::string lit_str;    // Utf8 literal bytes; also the pattern of E_STR_MATCH
   // E_BINARY
   BinOp op = OP_AND;
   // E_IN_LIST
   bool negated = false;
+  // E_STR_MATCH
+  StrMatch str_match = SM_STARTS_WITH;
   // E_CASE: children = [base?] w1 t1 w2 t2 ... [else]; flags say which are present
   bool case_has_base = false, case_has_else = false;
   std::vector<ExprP> children;

@@ -51,7 +51,7 @@ void check_keys(const std::vector<ExprP>& exprs, const char* what) {
 void check_data_schema(const SchemaDef& s, const char* what) {
   for (auto& f : s.fields) {
     const int w = f.type.byte_width();
-    if (f.type.id == T_BOOL || f.type.id == T_BINARY || f.type.id == T_NULL || w == 0)
+    if (f.type.id == T_BOOL || f.type.is_varlen() || f.type.id == T_NULL || w == 0)
       throw PlanError(B200Q_ERR_UNSUPPORTED, std::string(what) + ": a " + f.type.str() + " column in a join input is not on the GPU path");
   }
 }

@@ -78,6 +78,7 @@ struct FpSink {
       case PH_I32: ((int32_t*)v)[p] = (int32_t)lo; break;
       case PH_I64: case PH_F64: ((uint64_t*)v)[p] = lo; break;
       case PH_F32: ((float*)v)[p] = (float)as_f64(lo); break;
+      case PH_SEL: ((uint32_t*)v)[p] = (uint32_t)lo; break;
       default: ((uint64_t*)v)[2 * p] = lo; ((uint64_t*)v)[2 * p + 1] = hi; break;
     }
   }
@@ -916,6 +917,96 @@ int launch_exclusive_scan_i32(const int32_t* in, int32_t* out, int64_t n, int32_
   scan_sums_kernel<<<1, SCAN_BLOCK, 0, s>>>(d_block_sums, nb);
   scan_final_kernel<<<(unsigned)nb, SCAN_BLOCK, 0, s>>>(in, out, n, d_block_sums);
   return 3;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// variable-width gather (FilterExec / ProjectExec carrying Utf8 / Binary columns)
+// ---------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) varlen_lengths_kernel(const DevCol src, const uint32_t* __restrict__ sel, long long m, int32_t* __restrict__ lengths,
+                                                             uint32_t* __restrict__ out_valid, unsigned long long* __restrict__ total) {
+  const unsigned lane = threadIdx.x & 31;
+  unsigned long long sum = 0;
+  // 32 consecutive output rows per warp step: one validity word per step
+  for (long long base = (blockIdx.x * (long long)blockDim.x + threadIdx.x) & ~31LL; base < m; base += (long long)gridDim.x * blockDim.x) {
+    const long long i = base + lane;
+    bool valid = false;
+    if (i < m) {
+      const long long j = sel ? (long long)sel[i] : i;
+      const int32_t len = src.offsets[j + 1] - src.offsets[j];
+      lengths[i] = len; sum += (unsigned long long)len;
+      valid = true;
+      if (src.validity) { const unsigned long long bi = (unsigned long long)j + src.bit_offset; valid = (src.validity[bi >> 3] >> (bi & 7)) & 1; }
+    }
+    const unsigned w = __ballot_sync(0xffffffffu, valid);
+    if (out_valid && lane == 0) out_valid[base >> 5] = w;
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, d);
+  if (lane == 0 && sum) atomicAdd(total, sum);
+}
+
+struct alignas(16) V16 { unsigned long long lo, hi; };     // one 128-bit load / store
+
+// 16 output bytes from a source that is `m` (1..15) bytes past a 16-byte boundary: two aligned 16-byte loads, then each output word is
+// a funnel shift of two neighbouring source words
+__device__ __forceinline__ V16 shifted16(const V16* __restrict__ src, int v, unsigned m) {
+  const V16 a = src[v], b = src[v + 1];
+  const uint32_t w[8] = {(uint32_t)a.lo, (uint32_t)(a.lo >> 32), (uint32_t)a.hi, (uint32_t)(a.hi >> 32),
+                         (uint32_t)b.lo, (uint32_t)(b.lo >> 32), (uint32_t)b.hi, (uint32_t)(b.hi >> 32)};
+  const unsigned q = m >> 2, sh = (m & 3) * 8;
+  uint32_t x[5];
+#pragma unroll
+  for (int i = 0; i < 5; i++) x[i] = q == 0 ? w[i] : q == 1 ? w[i + 1] : q == 2 ? w[i + 2] : w[i + 3];
+  uint32_t o[4];
+#pragma unroll
+  for (int i = 0; i < 4; i++) o[i] = (uint32_t)(((((uint64_t)x[i + 1]) << 32) | x[i]) >> sh);
+  V16 r; r.lo = o[0] | ((unsigned long long)o[1] << 32); r.hi = o[2] | ((unsigned long long)o[3] << 32);
+  return r;
+}
+
+// One warp per group of 32 output rows; the rows are copied one after the other by the whole warp, so a long string spreads over
+// 32 lanes (and every warp of the grid keeps its own rows).  Strings of 64 bytes or more are stored as aligned 16-byte vectors: the
+// loads are aligned 16-byte vectors too, shifted into place when source and destination disagree modulo 16 (both loads of a lane hold
+// at least one byte of the string, so they stay inside its buffer).  Heads and tails are coalesced byte copies.
+__global__ void __launch_bounds__(256) varlen_copy_kernel(const DevCol src, const uint32_t* __restrict__ sel, long long m,
+                                                          const int32_t* __restrict__ out_offsets, uint8_t* __restrict__ out) {
+  const unsigned lane = threadIdx.x & 31;
+  const long long warps = ((long long)gridDim.x * blockDim.x) >> 5;
+  const uint8_t* data = (const uint8_t*)src.values;
+  for (long long base = ((blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5) * 32; base < m; base += warps * 32) {
+    const long long i = base + lane;
+    long long s0 = 0, d0 = 0; int len = 0;
+    if (i < m) { const long long j = sel ? (long long)sel[i] : i; s0 = src.offsets[j]; len = src.offsets[j + 1] - (int32_t)s0; d0 = out_offsets[i]; }
+    const int cnt = (int)(m - base < 32 ? m - base : 32);
+    for (int k = 0; k < cnt; k++) {
+      const uint8_t* sp = data + __shfl_sync(0xffffffffu, s0, k);
+      uint8_t* dp = out + __shfl_sync(0xffffffffu, d0, k);
+      const int n = __shfl_sync(0xffffffffu, len, k);
+      int done = 0;
+      if (n >= 64) {
+        const int head = (int)((16 - ((uintptr_t)dp & 15)) & 15);
+        if ((int)lane < head) dp[lane] = sp[lane];
+        const int nv = (n - head) >> 4;
+        const uint8_t* s = sp + head; V16* vd = (V16*)(dp + head);
+        const unsigned mis = (unsigned)((uintptr_t)s & 15);
+        if (mis == 0) { const V16* vs = (const V16*)s; for (int v = (int)lane; v < nv; v += 32) vd[v] = vs[v]; }
+        else { const V16* vs = (const V16*)(s - mis); for (int v = (int)lane; v < nv; v += 32) vd[v] = shifted16(vs, v, mis); }
+        done = head + (nv << 4);
+      }
+      for (int b = done + (int)lane; b < n; b += 32) dp[b] = sp[b];
+    }
+  }
+}
+
+int launch_varlen_lengths(const DevCol& src, const uint32_t* sel, int64_t m, int32_t* lengths, uint32_t* out_valid, unsigned long long* d_total, cudaStream_t s) {
+  if (m <= 0) return 0;
+  varlen_lengths_kernel<<<grid_for((m + 255) / 256, 8), 256, 0, s>>>(src, sel, m, lengths, out_valid, d_total);
+  return 1;
+}
+int launch_varlen_copy(const DevCol& src, const uint32_t* sel, int64_t m, const int32_t* out_offsets, uint8_t* out_data, cudaStream_t s) {
+  if (m <= 0) return 0;
+  varlen_copy_kernel<<<grid_for((m + 255) / 256, 8), 256, 0, s>>>(src, sel, m, out_offsets, out_data);
+  return 1;
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -119,4 +119,10 @@ int launch_frozen_read(const FrozenTable& ft, int64_t n, const int32_t* offsets,
 int launch_murmur3_partition(const ColTable& cols, const uint8_t* phys, int ncols, int64_t n, int32_t num_partitions, uint32_t* out, cudaStream_t s);
 int64_t scan_num_blocks(int64_t n);
 
+// variable-width (Utf8 / Binary) column gather: output row i is source row sel[i] (sel null: row i).  `src` is a DevCol whose
+// `offsets` are already advanced by the Arrow offset.  Pass 1 writes the lengths, the gathered validity bits (when `out_valid`)
+// and adds the total byte count to *d_total; pass 2 (after launch_exclusive_scan_i32 of the lengths) copies the bytes.
+int launch_varlen_lengths(const DevCol& src, const uint32_t* sel, int64_t m, int32_t* lengths, uint32_t* out_valid, unsigned long long* d_total, cudaStream_t s);
+int launch_varlen_copy(const DevCol& src, const uint32_t* sel, int64_t m, const int32_t* out_offsets, uint8_t* out_data, cudaStream_t s);
+
 }  // namespace b200q

@@ -20,7 +20,7 @@ std::string DType::str() const {
     case T_INT64: return "int64"; case T_FLOAT32: return "float32"; case T_FLOAT64: return "float64";
     case T_DATE32: return "date32"; case T_TIMESTAMP_US: return "timestamp[us]";
     case T_DECIMAL128: return "decimal128(" + std::to_string(precision) + "," + std::to_string(scale) + ")";
-    case T_BINARY: return "binary"; default: return "null";
+    case T_BINARY: return "binary"; case T_UTF8: return "utf8"; default: return "null";
   }
 }
 
@@ -101,7 +101,8 @@ DType parse_arrow_type(Reader r) {
         d = DType(); d.id = T_DECIMAL128; d.precision = (uint8_t)whole; d.scale = (int8_t)frac; set = true; break;
       }
       case 3: case 5: case 7: case 9: unsupported("unsigned integer columns are not on the hot path");
-      case 14: case 32: unsupported("Utf8 columns are not on the hot path (round 1)");
+      case 14: empty(T_UTF8); break;
+      case 32: unsupported("LargeUtf8 columns are not on the hot path");
       default: unsupported("ArrowType tag " + std::to_string(f) + " is not on the hot path");
     }
   }
@@ -160,7 +161,7 @@ ExprP wrap_try_cast(ExprP e, DType to) {
   return c;
 }
 
-void check_cast_supported(const DType& from, const DType& to);
+void check_cast_supported(const DType& from, const DType& to, bool try_cast);
 
 ExprP finish_binary(ExprP l, BinOp op, ExprP rr) {
   auto e = mk(E_BINARY); e->op = op; e->children = {l, rr};
@@ -216,6 +217,9 @@ ExprP parse_scalar_function(Reader r, const SchemaDef& schema) {   // PhysicalSc
     if (p < 1 || p > 38) bad(name + ": illegal precision");
     e->type.id = T_DECIMAL128; e->type.precision = (uint8_t)p; e->type.scale = (int8_t)s; return e;
   }
+  // NullIf / NullIfZero return their argument's value: over a string that is a string-valued expression, which stays off the device
+  if ((name == "NullIfZero" || name == "NullIf") && !args.empty() && args[0]->type.is_varlen())
+    unsupported(name + " over a " + args[0]->type.str() + " argument is not on the hot path");
   if (name == "NullIfZero") { if (args.size() != 1) bad("NullIfZero expects one argument"); e->type = args[0]->type; return e; }
   if (name == "NullIf") {
     if (args.size() != 2) bad("NullIf expects two arguments");
@@ -306,7 +310,7 @@ ExprP parse_expr(Reader r, const SchemaDef& schema) {
         Reader c = r.bytes(); ExprP ch; DType to; bool have_t = false;
         while (!c.done()) { int w; uint32_t g = c.tag(w); if (g == 1) ch = parse_expr(c.bytes(), schema); else if (g == 2) { to = parse_arrow_type(c.bytes()); have_t = true; } else c.skip(w); }
         if (!ch || !have_t) bad("Missing required field in protobuf");
-        check_cast_supported(ch->type, to);
+        check_cast_supported(ch->type, to, f == 15);
         auto e = mk(f == 10 ? E_CAST : E_TRY_CAST); e->children = {ch}; e->type = to;
         e->nullable = f == 10 ? ch->nullable : true;
         return e;
@@ -318,7 +322,7 @@ ExprP parse_expr(Reader r, const SchemaDef& schema) {
         auto e = mk(E_IN_LIST); e->negated = neg; e->children.push_back(x); e->type = bool_t(); e->nullable = x->nullable;
         for (auto& it : items) {
           ExprP item = it;
-          if (item->type != x->type) { check_cast_supported(item->type, x->type); item = wrap_try_cast(item, x->type); }   // from_proto.rs:888-895
+          if (item->type != x->type) { check_cast_supported(item->type, x->type, true); item = wrap_try_cast(item, x->type); }   // from_proto.rs:888-895
           e->nullable = e->nullable || item->nullable;
           e->children.push_back(item);
         }
@@ -335,7 +339,15 @@ ExprP parse_expr(Reader r, const SchemaDef& schema) {
       case 20: unsupported("LIKE is not on the hot path");
       case 10000: case 10001: unsupported("JVM-callback expressions (Spark UDF / scalar subquery wrappers) are not on the hot path");
       case 10002: case 10003: case 11000: unsupported("nested-type expressions are not on the hot path");
-      case 20000: case 20001: case 20002: unsupported("string expressions are not on the hot path");
+      case 20000: case 20001: case 20002: {   // StringStartsWith/EndsWith/ContainsExprNode{expr=1, prefix|suffix|infix=2} (auron.proto:339-352)
+        Reader c = r.bytes(); ExprP x; std::string pat;
+        while (!c.done()) { int w; uint32_t g = c.tag(w); if (g == 1) x = parse_expr(c.bytes(), schema); else if (g == 2) pat = c.str(); else c.skip(w); }
+        if (!x) bad("Missing required field in protobuf");
+        if (x->type.id != T_UTF8) bad("string match over a " + x->type.str() + " operand");
+        auto e = mk(E_STR_MATCH); e->children = {x}; e->lit_str = pat; e->str_match = (StrMatch)(f - 20000);
+        e->type = bool_t(); e->nullable = true;           // string_starts_with.rs:73-79
+        return e;
+      }
       case 20100: unsupported("RowNum is not on the hot path");
       case 20200: unsupported("BloomFilterMightContain is not on the hot path");
       default: r.skip(wt);
@@ -344,9 +356,12 @@ ExprP parse_expr(Reader r, const SchemaDef& schema) {
   bad("Unexpected empty physical expression");
 }
 
-void check_cast_supported(const DType& from, const DType& to) {
+// TryCast (the reference's TryCastExpr) from Utf8 to a signed integer is Spark's UTF8String.toLong; Cast (DataFusion CastExpr) from
+// Utf8 is arrow's parser with other semantics and stays off the device
+void check_cast_supported(const DType& from, const DType& to, bool try_cast) {
   if (from == to) return;
   if (from.id == T_NULL || to.id == T_NULL) return;
+  if (from.id == T_UTF8 && to.is_integer() && try_cast) return;
   auto num = [](const DType& t) { return t.is_integer() || t.is_float(); };
   bool ok = (num(from) && num(to)) || (from.id == T_BOOL && num(to)) || (num(from) && to.id == T_BOOL) ||
             (from.id == T_DATE32 && to.id == T_INT32) || (from.id == T_INT32 && to.id == T_DATE32) ||
@@ -446,7 +461,7 @@ PlanP parse_projection(Reader r) {           // ProjectionExecNode{input=1, expr
   size_t cnt = std::min(exprs.size(), std::min(names.size(), types.size()));   // zip semantics (from_proto.rs:126-129)
   for (size_t i = 0; i < cnt; i++) {
     ExprP e = parse_expr(exprs[i], n->input->schema);
-    if (e->type != types[i]) { check_cast_supported(e->type, types[i]); e = wrap_try_cast(e, types[i]); }   // from_proto.rs:133-137
+    if (e->type != types[i]) { check_cast_supported(e->type, types[i], true); e = wrap_try_cast(e, types[i]); }   // from_proto.rs:133-137
     n->proj_exprs.push_back(e);
     n->schema.fields.push_back(FieldDef{names[i], e->type, e->nullable});     // project_exec.rs:62-72
   }
@@ -476,7 +491,7 @@ PlanP parse_agg(Reader r) {                  // AggExecNode (auron.proto:675-685
   size_t ng = std::min(gexprs.size(), gnames.size());
   for (size_t i = 0; i < ng; i++) {
     ExprP e = parse_expr(gexprs[i], in);
-    if (e->type.id == T_BINARY || e->type.id == T_NULL) unsupported("grouping by " + e->type.str() + " is not on the hot path");
+    if (e->type.is_varlen() || e->type.id == T_NULL) unsupported("grouping by " + e->type.str() + " is not on the hot path");
     n->group_exprs.push_back(e); n->group_names.push_back(gnames[i]);
     n->schema.fields.push_back(FieldDef{gnames[i], e->type, e->nullable});    // agg_ctx.rs:91-101
   }
@@ -511,14 +526,15 @@ PlanP parse_agg(Reader r) {                  // AggExecNode (auron.proto:675-685
         a.data_type = rt;
         if (a.mode == MODE_PARTIAL) {
           if (!(rt.is_integer() || rt.id == T_FLOAT64 || rt.is_decimal())) unsupported("sum/avg accumulating at " + rt.str() + " is not on the hot path");
-          check_cast_supported(children[0]->type, rt);
+          if (children[0]->type.is_varlen()) unsupported(std::string(a.fn == AGG_SUM ? "sum" : "avg") + " over a " + children[0]->type.str() + " column is not on the hot path (cast it to a number first)");
+          check_cast_supported(children[0]->type, rt, true);
         }
         a.args.push_back(wrap_try_cast(children[0], rt));
       } else {
         a.data_type = a.mode == MODE_PARTIAL ? children[0]->type : children[0]->type;
         a.args.push_back(children[0]);
       }
-      if (a.data_type.id == T_BINARY || a.data_type.id == T_FLOAT32 && (a.fn == AGG_SUM || a.fn == AGG_AVG))
+      if (a.data_type.is_varlen() || a.data_type.id == T_FLOAT32 && (a.fn == AGG_SUM || a.fn == AGG_AVG))
         unsupported("aggregate over " + a.data_type.str() + " is not on the hot path");
     }
     n->aggs.push_back(a);
@@ -694,6 +710,7 @@ std::string explain_expr(const ExprP& e) {
       if (e->lit_null) o << "NULL";
       else if (e->type.is_float()) { double d; memcpy(&d, &e->lit_lo, 8); o << d; }
       else if (e->type.is_decimal()) { o << "dec(" << (int64_t)e->lit_hi << ":" << e->lit_lo << ")"; }
+      else if (e->type.id == T_UTF8) o << "'" << e->lit_str << "'";
       else o << (int64_t)e->lit_lo;
       o << ":" << e->type.str(); break;
     case E_BINARY: case E_SC_AND: case E_SC_OR:
@@ -706,6 +723,7 @@ std::string explain_expr(const ExprP& e) {
     case E_TRY_CAST: o << "TryCast(" << explain_expr(e->children[0]) << " AS " << e->type.str() << ")"; break;
     case E_CASE: { o << "Case("; for (size_t i = 0; i < e->children.size(); i++) o << (i ? ", " : "") << explain_expr(e->children[i]); o << ")"; break; }
     case E_IN_LIST: { o << explain_expr(e->children[0]) << (e->negated ? " NOT IN (" : " IN ("); for (size_t i = 1; i < e->children.size(); i++) o << (i > 1 ? ", " : "") << explain_expr(e->children[i]); o << ")"; break; }
+    case E_STR_MATCH: { static const char* nm[] = {"StartsWith", "EndsWith", "Contains"}; o << nm[e->str_match] << "(" << explain_expr(e->children[0]) << ", '" << e->lit_str << "')"; break; }
     case E_SCALAR_FN: { o << e->name << "("; for (size_t i = 0; i < e->children.size(); i++) o << (i ? ", " : "") << explain_expr(e->children[i]); o << ")"; break; }
   }
   return o.str();

@@ -59,7 +59,7 @@ class ShuffleWriteStage : public Stage, public ShuffleResult {
     uint32_t k8 = 0, kw = 0;
     for (size_t i = 0; i < in.fields.size(); i++) {
       const FieldDef& f = in.fields[i];
-      if (f.type.id == T_BINARY || f.type.id == T_NULL) throw PlanError(B200Q_ERR_UNSUPPORTED, "shuffle of a " + f.type.str() + " column is not on the GPU path");
+      if (f.type.is_varlen() || f.type.id == T_NULL) throw PlanError(B200Q_ERR_UNSUPPORTED, "shuffle of a " + f.type.str() + " column is not on the GPU path");
       ShufCol& c = base_.col[i];
       c.width = (uint8_t)f.type.byte_width(); c.nullable = f.nullable ? 1 : 0; c.k8 = k8; c.kw = kw;
       if (c.nullable) k8++;

@@ -34,7 +34,7 @@ class SortStage : public Stage {
       keys_.push_back(Key{se.expr->col_index, !se.asc, se.nulls_first});
     }
     for (auto& f : in.fields)
-      if (f.type.id == T_BOOL || f.type.id == T_BINARY || f.type.id == T_NULL) throw PlanError(B200Q_ERR_UNSUPPORTED, "SortExec over a " + f.type.str() + " column is not on the GPU path");
+      if (f.type.id == T_BOOL || f.type.is_varlen() || f.type.id == T_NULL) throw PlanError(B200Q_ERR_UNSUPPORTED, "SortExec over a " + f.type.str() + " column is not on the GPU path");
     fetch_ = node.sort_has_fetch ? (int64_t)node.sort_fetch : -1;
     for (size_t i = 0; i < in.fields.size(); i++) used_input_cols.push_back((int)i);
   }

@@ -66,9 +66,19 @@ static DevCol dev_col_of(const DevColumn& c) {
   DevCol d{};
   const int w = c.type.byte_width();
   d.values = c.values ? (const uint8_t*)c.values->ptr + (size_t)c.offset * (size_t)w : nullptr;
+  if (c.type.is_varlen()) d.offsets = c.offsets ? (const int32_t*)c.offsets->ptr + c.offset : nullptr;   // values: the data base the offsets index
   d.validity = c.validity ? (const uint8_t*)c.validity->ptr : nullptr;
   d.bit_offset = (uint32_t)c.offset;
   if (c.offset > 0xFFFFFFFFLL) throw ExecError(B200Q_ERR_UNSUPPORTED, "column offset beyond 2^32 rows");
+  return d;
+}
+
+// the program in device memory, its Utf8 constants relocated to their device addresses
+static DevMemP upload_program(const CompiledProgram& cp, cudaStream_t s) {
+  DevMemP d = DevMem::alloc(sizeof(VmProgram), s);
+  const VmProgram p = relocated_program(cp, d->ptr);
+  B200Q_CUDA(cudaMemcpyAsync(d->ptr, &p, sizeof(VmProgram), cudaMemcpyHostToDevice, s));
+  B200Q_CUDA(cudaStreamSynchronize(s));                 // `p` lives on this stack frame
   return d;
 }
 
@@ -88,6 +98,11 @@ class FilterProjectStage : public Stage {
   bool identity_ = false;            // no filter, output i = input column i: batches are forwarded as they are (no copy, no launch)
   bool lean_possible_ = false;
   LeanFpSpec lean_{};
+  // variable-width outputs (Utf8 / Binary column references): gathered from the input column, not evaluated by the VM program.
+  // out_src_[i] >= 0: output i is input column out_src_[i]; vm_out_[i]: index among the program's outputs otherwise
+  std::vector<int> out_src_, vm_out_;
+  bool varlen_ = false;
+  int sel_out_ = -1;                 // program output holding the source row of each survivor (filtered plans with varlen outputs)
 
   int slot_of(int col_index) const { for (size_t i = 0; i < cp_.used_cols.size(); i++) if (cp_.used_cols[i] == col_index) return (int)i; return -1; }
   static bool is_i64(const DType& t) { return t.id == T_INT64 || t.id == T_TIMESTAMP_US; }
@@ -128,12 +143,22 @@ class FilterProjectStage : public Stage {
     has_filters_ = !filters.empty();
     identity_ = !has_filters_ && outs.size() == in.fields.size();
     for (size_t i = 0; identity_ && i < outs.size(); i++) identity_ = outs[i]->kind == E_COLUMN && outs[i]->col_index == (int)i && outs[i]->type == in.fields[i].type;
-    cp_ = compile_program(filters, outs, has_filters_);
+    std::vector<ExprP> vm_outs;
+    for (const ExprP& o : outs) {
+      ExprP e = o;
+      while ((e->kind == E_TRY_CAST || e->kind == E_CAST) && e->children[0]->type == e->type) e = e->children[0];
+      if (!e->type.is_varlen()) { out_src_.push_back(-1); vm_out_.push_back((int)vm_outs.size()); vm_outs.push_back(o); continue; }
+      if (e->kind != E_COLUMN)
+        throw PlanError(B200Q_ERR_UNSUPPORTED, "ProjectExec: " + explain_expr(o) + " produces a " + e->type.str() + " value; only " + e->type.str() + " column references are on the hot path");
+      out_src_.push_back(e->col_index); vm_out_.push_back(-1);
+    }
+    varlen_ = vm_outs.size() != outs.size();
+    if (varlen_ && has_filters_) sel_out_ = (int)vm_outs.size();
+    cp_ = compile_program(filters, vm_outs, has_filters_, sel_out_);
     used_input_cols = cp_.used_cols;
-    if (!cx.conf.force_generic_kernels) detect_lean(filters, outs);
-    d_prog_ = DevMem::alloc(sizeof(VmProgram), cx.stream);
-    B200Q_CUDA(cudaMemcpyAsync(d_prog_->ptr, &cp_.prog, sizeof(VmProgram), cudaMemcpyHostToDevice, cx.stream));
-    B200Q_CUDA(cudaStreamSynchronize(cx.stream));
+    for (int c : out_src_) if (c >= 0 && std::find(used_input_cols.begin(), used_input_cols.end(), c) == used_input_cols.end()) used_input_cols.push_back(c);
+    if (!cx.conf.force_generic_kernels && !varlen_ && !cp_.has_strings) detect_lean(filters, outs);
+    d_prog_ = upload_program(cp_, cx.stream);
   }
 
   void push(OpContext& cx, DevBatch& in, std::vector<DevBatch>& outs) override {
@@ -159,6 +184,8 @@ class FilterProjectStage : public Stage {
       ot.values[i] = c.values->ptr; ot.validity[i] = c.validity ? (uint32_t*)c.validity->ptr : nullptr; ot.phys[i] = phys_of(od.type);
       ob.cols.push_back(c);
     }
+    DevMemP sel;
+    if (sel_out_ >= 0) { sel = DevMem::alloc((size_t)n * 4, cx.stream); ot.values[sel_out_] = sel->ptr; ot.validity[sel_out_] = nullptr; ot.phys[sel_out_] = PH_SEL; }
     bool lean = lean_possible_;
     for (size_t i = 0; lean && i < cp_.used_cols.size(); i++) lean = ct.col[i].validity == nullptr;
     DevMemP scratch = DevMem::alloc(32, cx.stream, true);
@@ -184,7 +211,54 @@ class FilterProjectStage : public Stage {
     { float ms = 0; B200Q_CUDA(cudaEventElapsedTime(&ms, cx.ev0, cx.ev1)); cx.m.gpu_ms += ms; if (cx.cur_stage == 0) { cx.m.hot_ms += ms; cx.m.hot_rows += n; cx.m.hot_launches++; } }
     check_device_error_flags((int)h[2]);
     ob.num_rows = (int64_t)h[1];
-    if (ob.num_rows > 0) outs.push_back(std::move(ob));       // sender.send drops empty batches (execution_context.rs:713-716)
+    if (ob.num_rows == 0) return;                            // sender.send drops empty batches (execution_context.rs:713-716)
+    if (!varlen_) { outs.push_back(std::move(ob)); return; }
+    DevBatch res; res.num_rows = ob.num_rows;
+    for (size_t i = 0; i < out_src_.size(); i++) res.cols.push_back(out_src_[i] < 0 ? ob.cols[(size_t)vm_out_[i]] : DevColumn());
+    gather_varlen(cx, in, sel ? (const uint32_t*)sel->ptr : nullptr, res);
+    outs.push_back(std::move(res));
+  }
+
+  // the Utf8 / Binary outputs of `res` = rows sel[0..m) (sel null: rows 0..m) of their input columns.  Lengths, validity and offsets
+  // of every column are computed first, so that one host round trip brings back all byte totals before the data is allocated.
+  void gather_varlen(OpContext& cx, const DevBatch& in, const uint32_t* sel, DevBatch& res) {
+    const int64_t m = res.num_rows;
+    auto ours = [](const DevMemP& p) { return !p || p->owned || p->owner; };           // borrowed caller memory (push_device) must be copied
+    struct Job { size_t out; DevCol src; };
+    std::vector<Job> jobs;
+    for (size_t i = 0; i < out_src_.size(); i++) {
+      if (out_src_[i] < 0) continue;
+      const DevColumn& c = in.cols[(size_t)out_src_[i]];
+      // no filter: share the buffers (imported offsets always start at 0, so the column indexes its own allocation)
+      if (!sel && c.offset == 0 && ours(c.values) && ours(c.offsets) && ours(c.validity)) { res.cols[i] = c; continue; }
+      jobs.push_back(Job{i, dev_col_of(c)});
+    }
+    if (jobs.empty()) return;
+    const size_t nj = jobs.size();
+    DevMemP totals = DevMem::alloc(nj * 8, cx.stream, true);
+    std::vector<DevMemP> keep;
+    for (size_t j = 0; j < nj; j++) {
+      DevColumn& o = res.cols[jobs[j].out];
+      const DevColumn& c = in.cols[(size_t)out_src_[jobs[j].out]];
+      o.type = c.type;
+      o.offsets = DevMem::alloc((size_t)(m + 1) * 4, cx.stream);
+      if (c.validity && out_schema.fields[jobs[j].out].nullable) o.validity = DevMem::alloc(bitmap_bytes(m), cx.stream);
+      DevMemP lengths = DevMem::alloc((size_t)m * 4 + 16, cx.stream), sums = DevMem::alloc((size_t)scan_num_blocks(m) * 4 + 16, cx.stream);
+      cx.m.launches += launch_varlen_lengths(jobs[j].src, sel, m, (int32_t*)lengths->ptr, o.validity ? (uint32_t*)o.validity->ptr : nullptr,
+                                             (unsigned long long*)totals->ptr + j, cx.stream);
+      cx.m.launches += launch_exclusive_scan_i32((const int32_t*)lengths->ptr, (int32_t*)o.offsets->ptr, m, (int32_t*)sums->ptr, cx.stream);
+      keep.push_back(lengths); keep.push_back(sums);                  // released stream-ordered after the scans
+    }
+    std::vector<unsigned long long> bytes(nj);
+    B200Q_CUDA(cudaMemcpyAsync(bytes.data(), totals->ptr, nj * 8, cudaMemcpyDeviceToHost, cx.stream));
+    B200Q_CUDA(cudaStreamSynchronize(cx.stream));
+    for (size_t j = 0; j < nj; j++) {
+      DevColumn& o = res.cols[jobs[j].out];
+      if (bytes[j] > 0x7FFFFFFFULL) throw ExecError(B200Q_ERR_UNSUPPORTED, "a " + o.type.str() + " output column of one batch exceeds 2 GiB (32-bit Arrow offsets); push smaller batches");
+      o.values = DevMem::alloc((size_t)bytes[j], cx.stream);
+      cx.m.launches += launch_varlen_copy(jobs[j].src, sel, m, (const int32_t*)o.offsets->ptr, (uint8_t*)o.values->ptr, cx.stream);
+    }
+    B200Q_CUDA(cudaGetLastError());
   }
   void finish(OpContext&, std::vector<DevBatch>&) override {}
 };
@@ -239,7 +313,8 @@ static bool same_expr(const ExprP& a, const ExprP& b) {
   if (a == b) return true;
   if (a->kind != b->kind || a->type != b->type || a->children.size() != b->children.size()) return false;
   if (a->kind == E_COLUMN) return a->col_index == b->col_index;
-  if (a->kind == E_LITERAL) return a->lit_null == b->lit_null && a->lit_lo == b->lit_lo && a->lit_hi == b->lit_hi;
+  if (a->kind == E_LITERAL) return a->lit_null == b->lit_null && a->lit_lo == b->lit_lo && a->lit_hi == b->lit_hi && a->lit_str == b->lit_str;
+  if (a->kind == E_STR_MATCH && (a->str_match != b->str_match || a->lit_str != b->lit_str)) return false;
   if (a->kind == E_BINARY && a->op != b->op) return false;
   if (a->kind == E_SCALAR_FN && a->name != b->name) return false;
   if (a->kind == E_IN_LIST && a->negated != b->negated) return false;
@@ -477,11 +552,12 @@ class AggStage : public Stage {
     if (merge_mode_ && !columnar_) used_input_cols.push_back(n_in_ - 1);
     std::sort(used_input_cols.begin(), used_input_cols.end());
     used_input_cols.erase(std::unique(used_input_cols.begin(), used_input_cols.end()), used_input_cols.end());
-    d_prog_ = DevMem::alloc(sizeof(VmProgram), cx.stream);
-    B200Q_CUDA(cudaMemcpyAsync(d_prog_->ptr, &cp_.prog, sizeof(VmProgram), cudaMemcpyHostToDevice, cx.stream));
+    d_prog_ = upload_program(cp_, cx.stream);
 
-    detect_fast(cx);
-    if (!fast_ok_) detect_wide(cx);
+    if (!cp_.has_strings) {                   // the specialised kernels read fixed-width columns only: string programs stay on the VM kernel
+      detect_fast(cx);
+      if (!fast_ok_) detect_wide(cx);
+    }
 
     // ---- frozen-row descriptors of the state columns (non-final output in the reference format)
     if (!final_) {

@@ -71,7 +71,107 @@ __device__ __forceinline__ bool sub_of(i128_t a, i128_t b, i128_t* r) {
   return (b >= 0) ? (*r > a) : (*r < a);
 }
 
+// ---- Utf8 helpers: {pointer, length} operands, bytes compared as uint8_t ----
+__device__ __forceinline__ int str_cmp(const uint8_t* a, uint32_t la, const uint8_t* b, uint32_t lb) {
+  const uint32_t m = la < lb ? la : lb;
+  for (uint32_t i = 0; i < m; i++) { const int d = (int)a[i] - (int)b[i]; if (d) return d; }
+  return la == lb ? 0 : (la < lb ? -1 : 1);                      // a proper prefix sorts first
+}
+__device__ __forceinline__ bool str_eq(const uint8_t* a, uint32_t la, const uint8_t* b, uint32_t lb) {
+  if (la != lb) return false;
+  for (uint32_t i = 0; i < la; i++) if (a[i] != b[i]) return false;
+  return true;
+}
+__device__ __forceinline__ bool str_contains(const uint8_t* s, uint32_t ls, const uint8_t* p, uint32_t lp) {
+  if (lp > ls) return false;
+  for (uint32_t i = 0; i + lp <= ls; i++) if (str_eq(s + i, lp, p, lp)) return true;
+  return false;
+}
+// Spark UTF8String.toLong / toInt as the reference ports it (commons cast.rs:287-361): no trimming, optional sign (a lone sign is
+// NULL), digits accumulated negatively and checked against the target width, a '.' ends the integral part and may only be
+// followed by digits, which are dropped; any other byte or an overflow is NULL.
+__device__ __forceinline__ bool str_to_int(const uint8_t* s, uint32_t n, int bits, int64_t* out) {
+  if (n == 0) return false;
+  const bool neg = s[0] == '-';
+  uint32_t i = 0;
+  if (neg || s[0] == '+') { i = 1; if (n == 1) return false; }
+  const int64_t mn = bits == 64 ? INT64_MIN : -(1LL << (bits - 1)), stop = mn / 10;
+  int64_t r = 0;
+  while (i < n) {
+    const uint8_t b = s[i++];
+    if (b == '.') break;
+    if (b < '0' || b > '9') return false;
+    if (r < stop) return false;
+    r = sext((int64_t)((uint64_t)r * 10u - (uint64_t)(b - '0')), bits);   // wraps like the target type
+    if (r > 0) return false;
+  }
+  for (; i < n; i++) if (s[i] < '0' || s[i] > '9') return false;
+  if (!neg) { r = sext((int64_t)(0 - (uint64_t)r), bits); if (r < 0) return false; }
+  *out = r;
+  return true;
+}
+#define STRP(x) ((const uint8_t*)(uintptr_t)(x))
+
 struct NullSink { template <class... A> __device__ void out(A...) {} };
+
+#define VALID(r, i) ((vm[r] >> (i)) & 1u)
+#define SETV(r, i, ok) vm[r] = (vm[r] & ~(1u << (i))) | ((uint32_t)((ok) ? 1u : 0u) << (i))
+#define FORR _Pragma("unroll") for (int r = 0; r < R; r++)
+
+// The Utf8 instructions (VM_CMP_STR, VM_STARTS_WITH / ENDS_WITH / CONTAINS, VM_CAST_STR_I, VM_IN_LIST kind 3).  Returns the new
+// stack pointer.
+template <int R>
+__device__ __forceinline__ int vm_str(const VmInstr in, const uint64_t* __restrict__ pool, uint64_t (&st)[VM_MAX_DEPTH][R], uint32_t (&vm)[R], int sp) {
+  switch (in.op) {
+    case VM_CMP_STR: {
+      sp -= 3;
+      FORR {
+        const bool ok = VALID(r, sp - 1) && VALID(r, sp + 1);
+        const int c = ok ? str_cmp(STRP(st[sp - 1][r]), (uint32_t)st[sp][r], STRP(st[sp + 1][r]), (uint32_t)st[sp + 2][r]) : 0;
+        bool v;
+        switch (in.a) { case CMP_EQ: v = c == 0; break; case CMP_NE: v = c != 0; break; case CMP_LT: v = c < 0; break;
+                        case CMP_LE: v = c <= 0; break; case CMP_GT: v = c > 0; break; default: v = c >= 0; }
+        st[sp - 1][r] = v; SETV(r, sp - 1, ok);
+      }
+      return sp;
+    }
+    case VM_STARTS_WITH: case VM_ENDS_WITH: case VM_CONTAINS: {
+      sp -= 3;
+      FORR {
+        const bool ok = VALID(r, sp - 1);
+        const uint8_t* s = STRP(st[sp - 1][r]); const uint32_t ls = (uint32_t)st[sp][r];
+        const uint8_t* p = STRP(st[sp + 1][r]); const uint32_t lp = (uint32_t)st[sp + 2][r];
+        bool v = false;
+        if (ok) {
+          if (in.op == VM_CONTAINS) v = str_contains(s, ls, p, lp);
+          else v = lp <= ls && str_eq(in.op == VM_STARTS_WITH ? s : s + (ls - lp), lp, p, lp);
+        }
+        st[sp - 1][r] = v; SETV(r, sp - 1, ok);
+      }
+      return sp;
+    }
+    case VM_CAST_STR_I: {
+      sp -= 1;
+      FORR {
+        int64_t v = 0;
+        const bool ok = VALID(r, sp - 1) && str_to_int(STRP(st[sp - 1][r]), (uint32_t)st[sp][r], in.a, &v);
+        st[sp - 1][r] = ok ? (uint64_t)v : 0; SETV(r, sp - 1, ok);
+      }
+      return sp;
+    }
+    default: {                     // VM_IN_LIST over Utf8
+      const bool neg = in.a & 4, has_null = in.a & 8;
+      const int ix = sp - 2;
+      FORR {
+        bool found = false;
+        if (VALID(r, ix)) for (int k = 0; k < in.b && !found; k++) found = str_eq(STRP(st[ix][r]), (uint32_t)st[ix + 1][r], STRP(pool[in.c + 2 * k]), (uint32_t)pool[in.c + 2 * k + 1]);
+        const bool ok = VALID(r, ix) && (found || !has_null);
+        st[ix][r] = found != neg; SETV(r, ix, ok);
+      }
+      return ix + 1;
+    }
+  }
+}
 
 // Runs from `pc` until VM_END (returns -1) or VM_COMPACT (returns the pc after it).
 template <int R, class Sink>
@@ -83,10 +183,6 @@ __device__ __forceinline__ int vm_run(const VmInstr* __restrict__ code, const ui
   int sp = 0;
 #pragma unroll
   for (int r = 0; r < R; r++) vm[r] = 0;
-
-#define VALID(r, i) ((vm[r] >> (i)) & 1u)
-#define SETV(r, i, ok) vm[r] = (vm[r] & ~(1u << (i))) | ((uint32_t)((ok) ? 1u : 0u) << (i))
-#define FORR _Pragma("unroll") for (int r = 0; r < R; r++)
 
   while (true) {
     const VmInstr in = code[pc++];
@@ -116,6 +212,22 @@ __device__ __forceinline__ int vm_run(const VmInstr* __restrict__ code, const ui
           if (in.a == PH_DEC128) st[sp + 1][r] = hi;
         }
         sp += in.a == PH_DEC128 ? 2 : 1;
+        break;
+      }
+      case VM_LOAD_STR: {          // Utf8 column -> {pointer into the data, length}
+        const DevCol c = cols.col[in.b];
+        FORR {
+          uint64_t p = 0, len = 0; bool ok = false;
+          if (inb[r]) {
+            const long long i = row[r];
+            ok = true;
+            if (c.validity) { const unsigned long long bi = (unsigned long long)i + c.bit_offset; ok = (__ldg(c.validity + (bi >> 3)) >> (bi & 7)) & 1; }
+            const int32_t o0 = __ldg(c.offsets + i), o1 = __ldg(c.offsets + i + 1);
+            p = (uint64_t)(uintptr_t)((const uint8_t*)c.values + o0); len = (uint64_t)(uint32_t)(o1 - o0);
+          }
+          st[sp][r] = p; st[sp + 1][r] = len; SETV(r, sp, ok);
+        }
+        sp += 2;
         break;
       }
       case VM_LOAD_LIT: {
@@ -372,8 +484,9 @@ __device__ __forceinline__ int vm_run(const VmInstr* __restrict__ code, const ui
         break;
       }
       case VM_IN_LIST: {
+        if ((in.a & 3) == 3) { sp = vm_str<R>(in, pool, st, vm, sp); break; }
         const int kind = in.a & 3; const bool neg = in.a & 4, has_null = in.a & 8;
-        const int n = kind == 2 ? 2 : 1, ix = sp - n;
+        const int n = kind >= 2 ? 2 : 1, ix = sp - n;
         FORR {
           bool found = false;
           if (kind == 2) { for (int k = 0; k < in.b; k++) found |= pool[in.c + 2 * k] == st[ix][r] && pool[in.c + 2 * k + 1] == st[ix + 1][r]; }
@@ -391,14 +504,17 @@ __device__ __forceinline__ int vm_run(const VmInstr* __restrict__ code, const ui
         break;
       }
       case VM_OUT: {
-        const int n = in.a == PH_DEC128 ? 2 : 1;
+        const int n = in.a >= PH_DEC128 ? 2 : 1;
         sp -= n;
         FORR { sink.out(r, (int)in.b, (int)in.a, st[sp][r], n == 2 ? st[sp + 1][r] : 0ULL, (bool)VALID(r, sp)); }
         break;
       }
+      case VM_OUT_SEL: FORR { sink.out(r, (int)in.b, (int)PH_SEL, (uint64_t)row[r], 0ULL, true); } break;
+      case VM_CMP_STR: case VM_STARTS_WITH: case VM_ENDS_WITH: case VM_CONTAINS: case VM_CAST_STR_I: sp = vm_str<R>(in, pool, st, vm, sp); break;
       default: return -1;
     }
   }
+#undef STRP
 #undef VALID
 #undef SETV
 #undef FORR

@@ -4,7 +4,8 @@
 // each — CachedExprsEvaluator::filter_impl, cached_exprs_evaluator.rs:90-136), then the projections /
 // grouping keys / aggregate arguments (VM_OUT).  It is a typed stack machine: every value is one
 // 64-bit slot (ints/bool/date/timestamp sign-extended to i64; f32/f64 as an f64) or two slots
-// (decimal128 lo,hi) plus one validity bit per slot.  There is no control flow: CASE compiles to
+// (decimal128 lo,hi; a Utf8 string {byte pointer, length}) plus one validity bit per slot (a two-slot
+// value's validity is the bit of its first slot).  There is no control flow: CASE compiles to
 // VM_SELECT, so R rows per thread run in lockstep and the program counter is warp-uniform.
 #pragma once
 #include <cstdint>
@@ -40,13 +41,20 @@ enum VmOp : uint8_t {
   VM_NULLIFY,         // a = value slots: pops bool m, value v -> v with validity cleared where m is true
   VM_NORM_NAN_ZERO,   // a = 1: f32
   VM_SELECT,          // a = value slots: pops else, then, cond -> (cond valid && true) ? then : else
-  VM_IN_LIST,         // a = bits: 0-1 kind (0 int,1 float,2 dec), bit2 negated, bit3 list has a NULL item; b = count; c = pool index
+  VM_IN_LIST,         // a = bits: 0-1 kind (0 int,1 float,2 dec,3 utf8), bit2 negated, bit3 list has a NULL item; b = count; c = pool index
   VM_FILTER,          // pops bool: row stays alive iff valid && true (null -> false, :518-520)
   VM_COMPACT,         // FilterExec/ProjectExec kernel only: all predicates done, compute output positions
   VM_OUT,             // a = OutKind, b = output index: pops the value
+  // Utf8 (operands are {pointer, length} pairs; byte loops run inside one instruction, the pc stays warp-uniform)
+  VM_CMP_STR,         // a = CmpOp: unsigned byte-lexicographic, a proper prefix sorts first (arrow Utf8 cmp)
+  VM_STARTS_WITH, VM_ENDS_WITH, VM_CONTAINS,               // pops pattern, string -> bool; an empty pattern matches
+  VM_CAST_STR_I,      // a = target bits: Spark UTF8String.toLong/toInt (commons cast.rs:287-361); NULL on bad input
+  VM_LOAD_STR,        // b = column slot: pushes {pointer into the data, length} of a Utf8 column
+  VM_OUT_SEL,         // b = output index: the source row of the (surviving) row, for the variable-width gathers
 };
 
-enum PhysKind : uint8_t { PH_BOOL = 0, PH_I8, PH_I16, PH_I32, PH_I64, PH_F32, PH_F64, PH_DEC128 };
+enum PhysKind : uint8_t { PH_BOOL = 0, PH_I8, PH_I16, PH_I32, PH_I64, PH_F32, PH_F64, PH_DEC128, PH_STR,
+                          PH_SEL };   // VM_OUT_SEL's output: the u32 source row of each surviving row
 enum CmpOp : uint8_t { CMP_EQ = 0, CMP_NE, CMP_LT, CMP_LE, CMP_GT, CMP_GE };
 
 struct VmInstr { uint8_t op, a; uint16_t b; uint32_t c; };
@@ -57,11 +65,15 @@ constexpr int VM_MAX_POOL = 256;
 constexpr int VM_MAX_DEPTH = 16;
 constexpr int VM_MAX_COLS = 32;     // distinct input columns referenced by one program
 constexpr int VM_MAX_OUT = 32;      // outputs (projection columns, or key words + agg args)
+constexpr int VM_MAX_STR_POOL = 4096;   // bytes of Utf8 literals, patterns and IN-list items per program
 
 struct VmProgram {
   uint32_t n_code, n_pool, n_filters, max_depth;
   VmInstr code[VM_MAX_CODE];
   uint64_t pool[VM_MAX_POOL];
+  // Utf8 constants: the pool holds {device address into str_pool, length} pairs for them (relocated at upload)
+  uint32_t n_str, _pad;
+  uint8_t str_pool[VM_MAX_STR_POOL];
 };
 
 // One input column as seen by a kernel launch (Arrow buffers; `validity` may be null).
@@ -70,6 +82,7 @@ struct DevCol {
   const uint8_t* validity;   // bit-packed, LSB first
   uint32_t bit_offset;       // Arrow offset for validity (and for bit-packed bool values)
   uint32_t _pad;
+  const int32_t* offsets;    // Utf8 / Binary: Arrow offsets advanced by the Arrow offset; they index `values` (the data base)
 };
 struct ColTable { DevCol col[VM_MAX_COLS]; };
 

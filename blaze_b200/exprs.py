@@ -235,6 +235,31 @@ class SCOr(Expr):
     def nullable(self, schema): return self.left.nullable(schema) or self.right.nullable(schema)
 
 
+@dataclass(frozen=True)
+class StringMatch(Expr):
+    """`StringStartsWithExprNode{expr, prefix}` / `StringEndsWithExprNode{expr, suffix}` / `StringContainsExprNode{expr, infix}`
+    (auron.proto:339-352): Boolean, always nullable (datafusion-ext-exprs/src/string_starts_with.rs:73-79)."""
+    kind: str            # "StartsWith" | "EndsWith" | "Contains"
+    expr: Expr
+    pattern: str
+
+    def __post_init__(self):
+        if self.kind not in STRING_MATCH_KINDS:
+            raise ValueError(f"unknown string match {self.kind!r}")
+
+    def children(self): return (self.expr,)
+    def data_type(self, schema): return T.bool_
+    def nullable(self, schema): return True
+
+
+STRING_MATCH_KINDS = ("StartsWith", "EndsWith", "Contains")
+
+
+def StartsWith(expr: Expr, prefix: str) -> StringMatch: return StringMatch("StartsWith", expr, prefix)
+def EndsWith(expr: Expr, suffix: str) -> StringMatch: return StringMatch("EndsWith", expr, suffix)
+def Contains(expr: Expr, infix: str) -> StringMatch: return StringMatch("Contains", expr, infix)
+
+
 # Spark ext functions on the hot path (datafusion-ext-functions/src/lib.rs:34-68)
 SPARK_EXT_FUNCTIONS = ("UnscaledValue", "MakeDecimal", "CheckOverflow", "NullIfZero", "NullIf",
                        "NormalizeNanAndZero", "Placeholder")

@@ -187,7 +187,8 @@ _RELEASE_CB = C.CFUNCTYPE(None, C.POINTER(ArrowArray))
 class DeviceBatch:
     """A struct-typed ArrowDeviceArray over device pointers (torch tensors or raw addresses).
 
-    columns: list of (values_ptr, validity_ptr_or_0, length) for fixed-width columns.
+    columns: list of (values_ptr, validity_ptr_or_0, length) for fixed-width columns, and
+    (data_ptr, validity_ptr_or_0, length, offsets_ptr) for Utf8 / Binary columns (int32 Arrow offsets).
     `keepalive` objects (the tensors) are held until the library calls release.
     """
     _live = {}
@@ -198,11 +199,12 @@ class DeviceBatch:
         self.children = (ArrowArray * self.n)()
         self.child_ptrs = (C.POINTER(ArrowArray) * self.n)()
         self.buffers = []
-        for i, (vptr, nptr, ln) in enumerate(columns):
-            b = (C.c_void_p * 2)(nptr or None, vptr)
+        for i, col in enumerate(columns):
+            vptr, nptr, ln = col[:3]
+            b = (C.c_void_p * 3)(nptr or None, col[3], vptr) if len(col) == 4 else (C.c_void_p * 2)(nptr or None, vptr)
             self.buffers.append(b)
             c = self.children[i]
-            c.length, c.null_count, c.offset, c.n_buffers, c.n_children = ln, (-1 if nptr else 0), 0, 2, 0
+            c.length, c.null_count, c.offset, c.n_buffers, c.n_children = ln, (-1 if nptr else 0), 0, len(b), 0
             c.buffers = C.cast(b, C.POINTER(C.c_void_p))
             c.release = C.cast(_noop_release, C.c_void_p)
             self.child_ptrs[i] = C.pointer(c)

@@ -10,12 +10,12 @@ from __future__ import annotations
 from dataclasses import dataclass
 
 # type ids shared with the C ABI (include/blaze_b200.h: b200q_type_id)
-BOOL, INT8, INT16, INT32, INT64, FLOAT32, FLOAT64, DATE32, TIMESTAMP_US, DECIMAL128, BINARY, NULLTYPE = range(12)
+BOOL, INT8, INT16, INT32, INT64, FLOAT32, FLOAT64, DATE32, TIMESTAMP_US, DECIMAL128, BINARY, NULLTYPE, UTF8 = range(13)
 
 _NAMES = {
     BOOL: "bool", INT8: "int8", INT16: "int16", INT32: "int32", INT64: "int64",
     FLOAT32: "float32", FLOAT64: "float64", DATE32: "date32", TIMESTAMP_US: "timestamp[us]",
-    DECIMAL128: "decimal128", BINARY: "binary", NULLTYPE: "null",
+    DECIMAL128: "decimal128", BINARY: "binary", NULLTYPE: "null", UTF8: "utf8",
 }
 
 
@@ -62,6 +62,7 @@ float64 = DataType(FLOAT64)
 date32 = DataType(DATE32)
 timestamp_us = DataType(TIMESTAMP_US)
 binary = DataType(BINARY)
+utf8 = DataType(UTF8)
 null = DataType(NULLTYPE)
 
 
@@ -118,6 +119,7 @@ def from_arrow_type(t) -> DataType:
         return timestamp_us
     if pa.types.is_decimal128(t): return decimal128(t.precision, t.scale)
     if pa.types.is_binary(t): return binary
+    if pa.types.is_string(t): return utf8
     if pa.types.is_null(t): return null
     raise TypeError(f"unsupported arrow type on the hot path: {t}")
 
@@ -127,7 +129,7 @@ def to_arrow_type(dt: DataType):
     return {
         BOOL: pa.bool_(), INT8: pa.int8(), INT16: pa.int16(), INT32: pa.int32(), INT64: pa.int64(),
         FLOAT32: pa.float32(), FLOAT64: pa.float64(), DATE32: pa.date32(),
-        TIMESTAMP_US: pa.timestamp("us"), BINARY: pa.binary(), NULLTYPE: pa.null(),
+        TIMESTAMP_US: pa.timestamp("us"), BINARY: pa.binary(), NULLTYPE: pa.null(), UTF8: pa.string(),
     }[dt.id] if dt.id != DECIMAL128 else pa.decimal128(dt.precision, dt.scale)
 
 

@@ -232,3 +232,122 @@ def run_parquet(name, compression, n_pq):
 
 run_parquet("M6 parquet scan store_sales-like 4 columns, snappy + dictionary", "snappy", 1 << 24)
 run_parquet("M6 parquet scan store_sales-like 4 columns, uncompressed", "none", 1 << 24)
+
+
+# S1-S3: Utf8 columns (device-resident, generated from the seed: lengths -> cumsum offsets, bytes from a table); 2^26 rows unless ROWS is
+# set: one batch of a Utf8 column holds at most 2 GiB (32-bit Arrow offsets), and 2^26 rows of nm (mean 20 B) are 1.3 GB.  Algorithmic bytes are counted from the generated buffers: every input byte read once (values, offsets, data) plus every output byte
+# written once (offsets included), so they follow the data rather than a per-row constant.
+srows = int(os.environ.get("ROWS", 1 << 26))
+
+
+def utf8_column(lengths, lo, span):
+    """offsets from the lengths; bytes uniform in [lo, lo + span)"""
+    offs = torch.zeros(lengths.numel() + 1, dtype=torch.int32, device=dev)
+    offs[1:] = torch.cumsum(lengths, 0).to(torch.int32)
+    data = torch.randint(lo, lo + span, (int(offs[-1].item()),), dtype=torch.uint8, device=dev, generator=g)
+    return data, offs
+
+
+def run_strings(name, plan, cols, in_bytes, check):
+    """cols: [tensor] for fixed width, [(data, offsets)] for Utf8; check(out_batches_on_host) verifies and returns the output bytes.
+    Timed: push_device -> finish -> sync (every kernel of the op, no host export)."""
+    if ONLY and not any(t in name for t in ONLY.split(",")): return
+    import time
+    spec, keep = [], []
+    for c in cols:
+        if isinstance(c, tuple): spec.append((c[0].data_ptr(), 0, srows, c[1].data_ptr())); keep += list(c)
+        else: spec.append((c.data_ptr(), 0, srows)); keep.append(c)
+    best = None
+    for _ in range(REPS or 3):
+        with native.NativeOp(plan.plan_bytes(), native.default_conf(agg_initial_groups=1 << 20), 0) as op:
+            torch.cuda.synchronize(); t0 = time.perf_counter()
+            op.push_device(native.DeviceBatch(spec, srows, 0, keepalive=keep))
+            op.finish(); op.sync()
+            dt = time.perf_counter() - t0
+            m = op.metrics()
+            outs = op.pull_all()
+        if best is None or dt < best[0]: best = (dt, m, outs)
+        del outs
+    dt, m, outs = best
+    out_bytes = check(outs)
+    gbs = (in_bytes + out_bytes) / dt / 1e9
+    print(json.dumps({"shape": name, "rows": srows, "out_rows": sum(b.num_rows for b in outs), "wall_ms_push_to_sync": dt * 1e3, "rows_per_s": srows / dt,
+                      "alg_bytes": in_bytes + out_bytes, "alg_GBps": gbs, "frac_of_hbm_peak": gbs / peak, "launches": m["gpu_kernel_launches"]}), flush=True)
+
+
+def contains_rows(data, offs, pat):
+    """per row: does the string hold `pat` (torch; positions of the first byte, then a search over the offsets)"""
+    hit = torch.ones(data.numel() - len(pat) + 1, dtype=torch.bool, device=dev)
+    for j, ch in enumerate(pat.encode()):
+        hit &= data[j: data.numel() - len(pat) + 1 + j] == ch
+    at = hit.nonzero().squeeze(1)
+    row = torch.searchsorted(offs.long(), at, right=True) - 1
+    ok = at + len(pat) <= offs.long()[row + 1]
+    out = torch.zeros(offs.numel() - 1, dtype=torch.bool, device=dev)
+    out[row[ok]] = True
+    return out
+
+
+if any(t in (ONLY or "S1,S2,S3") for t in ("S1", "S2", "S3")):
+    import numpy as np
+    codes = [a + b for a in "abcdefghij" for b in "abcde"]                   # 50 two-letter codes
+    pick = torch.randint(0, 50, (srows,), device=dev, generator=g)
+    code_bytes = torch.tensor([[ord(c[0]), ord(c[1])] for c in codes], dtype=torch.uint8, device=dev)
+    st_data, st_offs = code_bytes[pick].reshape(-1).contiguous(), torch.arange(0, 2 * srows + 1, 2, dtype=torch.int32, device=dev)
+    nm_len = torch.randint(8, 33, (srows,), device=dev, generator=g)
+    nm_data, nm_offs = utf8_column(nm_len, ord("a"), 26)
+    kk = torch.arange(srows, dtype=torch.int64, device=dev)
+    s_sch = T.Schema([T.Field("k", T.int64, False), T.Field("st", T.utf8, False), T.Field("nm", T.utf8, False)])
+
+    def carried_check(mask):
+        def check(outs):
+            want_rows = int(mask.sum().item())
+            assert sum(b.num_rows for b in outs) == want_rows, "row count differs from the torch computation"
+            got_k = np.concatenate([b.column("k").to_numpy() for b in outs]) if outs else np.zeros(0, np.int64)
+            assert np.array_equal(got_k, kk[mask].cpu().numpy()), "carried keys differ"
+            got_sum = 0
+            for b in outs:
+                c = b.column("nm")
+                o = np.frombuffer(c.buffers()[1], np.int32)[c.offset: c.offset + len(c) + 1]
+                got_sum += int(np.frombuffer(c.buffers()[2], np.uint8)[o[0]:o[-1]].astype(np.int64).sum())
+            assert got_sum == int(nm_data[torch.repeat_interleave(mask, nm_len)].to(torch.int64).sum().item()), "checksum of the carried bytes differs"
+            return 8 * want_rows + 4 * (want_rows + 1) + int(nm_len[mask].sum().item())
+        return check
+
+    in_s12 = 8 * srows + (st_offs.numel() + nm_offs.numel()) * 4 + st_data.numel() + nm_data.numel()
+    chosen = ["ab", "cd", "fa", "je"]
+    s1 = PL.ProjectExec([(E.Column("k"), "k"), (E.Column("nm"), "nm")],
+                        PL.FilterExec([E.InList(E.Column("st"), [E.Literal(c, T.utf8) for c in chosen])], PL.MemoryExec(s_sch)))
+    run_strings("S1 Filter[st IN (4 of 50)] -> Project[k, nm]", s1, [kk, (st_data, st_offs), (nm_data, nm_offs)], in_s12,
+                carried_check(torch.isin(pick, torch.tensor([codes.index(c) for c in chosen], device=dev))))
+    s2 = PL.ProjectExec([(E.Column("k"), "k"), (E.Column("nm"), "nm")],
+                        PL.FilterExec([E.BinaryExpr(E.StartsWith(E.Column("nm"), "ab"), "Or", E.Contains(E.Column("nm"), "xyz"))], PL.MemoryExec(s_sch)))
+    starts = (nm_data[nm_offs[:-1].long()] == ord("a")) & (nm_data[nm_offs[:-1].long() + 1] == ord("b"))
+    run_strings("S2 Filter[StartsWith(nm,'ab') OR Contains(nm,'xyz')] -> Project[k, nm]", s2, [kk, (st_data, st_offs), (nm_data, nm_offs)], in_s12,
+                carried_check(starts | contains_rows(nm_data, nm_offs, "xyz")))
+    del st_data, st_offs, nm_data, nm_offs, pick, kk, starts
+    # S3: SUM(TryCast(ns AS BIGINT)) GROUP BY k over 1-12-digit numeric strings, 1 % junk (a letter as the first byte)
+    ns_len = torch.randint(1, 13, (srows,), device=dev, generator=g)
+    ns_data, ns_offs = utf8_column(ns_len, ord("0"), 10)
+    junk = torch.rand(srows, device=dev, generator=g) < 0.01
+    ns_data[ns_offs[:-1].long()[junk]] = ord("q")
+    kg = torch.randint(0, 1 << 16, (srows,), dtype=torch.int64, device=dev, generator=g)
+    s3_sch = T.Schema([T.Field("k", T.int64, False), T.Field("ns", T.utf8, False)])
+    sum_of = lambda mode: [E.AggExpr("s", mode, PL.create_agg(E.AGG_SUM, [E.TryCast(E.Column("ns"), T.int64) if mode == E.PARTIAL else E.placeholder(T.int64)], s3_sch, T.int64))]
+    s3 = PL.AggExec(PL.HashAgg, [E.GroupingExpr("k", E.Column("k"))], sum_of(E.FINAL), False,
+                    PL.AggExec(PL.HashAgg, [E.GroupingExpr("k", E.Column("k"))], sum_of(E.PARTIAL), False, PL.MemoryExec(s3_sch)))
+    val = torch.zeros(srows, dtype=torch.int64, device=dev)                      # torch reference: the decimal value of each string
+    start = ns_offs[:-1].long()
+    for p in range(12):
+        live = ns_len > p
+        val = torch.where(live, val * 10 + (ns_data[torch.where(live, start + p, start)].to(torch.int64) - ord("0")), val)
+    val[junk] = 0
+    want = torch.zeros(1 << 16, dtype=torch.int64, device=dev).index_add_(0, kg, val).cpu().numpy()
+    groups = int((torch.bincount(kg, minlength=1 << 16) > 0).sum().item())
+    del val, start
+
+    def s3_check(outs):
+        got = {int(k): int(s) for b in outs for k, s in zip(b.column("k").to_numpy(), b.column("s").to_numpy())}
+        assert len(got) == groups and all(got[k] == int(want[k]) for k in got), "S3 sums differ from the torch computation"
+        return 16 * len(got)
+    run_strings("S3 SUM(TryCast(ns AS BIGINT)) GROUP BY k", s3, [kg, (ns_data, ns_offs)], 8 * srows + ns_offs.numel() * 4 + ns_data.numel(), s3_check)

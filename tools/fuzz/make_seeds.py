@@ -24,7 +24,17 @@ def seed_plans():
     specs = [(E.AGG_SUM, D, T.decimal128(27, 2)), (E.AGG_COUNT, X, T.int64), (E.AGG_MAX, X, T.float64), (E.AGG_AVG, A, T.float64), (E.AGG_MIN, B, T.int32)]
     fin = [E.AggExpr(a.field_name, E.FINAL, PL.create_agg(fn, [E.placeholder(ch.data_type(s))], partial.schema(), rt)) for a, (fn, ch, rt) in zip(aggs, specs)]
     final = PL.AggExec(PL.HashAgg, [E.GroupingExpr("a", A), E.GroupingExpr("b", B)], fin, False, partial)
-    return [proj.plan_bytes(), partial.plan_bytes(), final.plan_bytes()]
+    # Utf8: string nodes, comparisons, IN lists, TryCast(Utf8 -> int), COUNT / SUM(TryCast) over a string column
+    su = T.Schema([T.Field("k", T.int64, False), T.Field("s", T.utf8, True), T.Field("t", T.utf8, True)])
+    S_, T_ = E.Column("s"), E.Column("t")
+    fs = PL.FilterExec([E.StartsWith(S_, "ab"), E.SCOr(E.EndsWith(S_, "é"), E.Contains(T_, "")), E.BinaryExpr(S_, "LtEq", T_),
+                        E.InList(S_, [E.Literal("x", T.utf8), E.Literal(None, T.utf8), E.Literal("", T.utf8)], True),
+                        E.BinaryExpr(E.Literal("b", T.utf8), "NotEq", S_), E.IsNotNull(T_)], PL.MemoryExec(su))
+    ps = PL.ProjectExec([(E.Column("k"), "k"), (S_, "s"), (E.TryCast(T_, T.int32), "ti")], fs)
+    sa = PL.AggExec(PL.HashAgg, [E.GroupingExpr("k", E.Column("k"))],
+                    [E.AggExpr("c", E.PARTIAL, PL.create_agg(E.AGG_COUNT, [S_], su, T.int64)),
+                     E.AggExpr("n", E.PARTIAL, PL.create_agg(E.AGG_SUM, [E.TryCast(T_, T.int64)], su, T.int64))], False, fs)
+    return [proj.plan_bytes(), partial.plan_bytes(), final.plan_bytes(), ps.plan_bytes(), sa.plan_bytes()]
 
 
 if __name__ == "__main__":
@@ -35,6 +45,7 @@ if __name__ == "__main__":
     import decimal
     from blaze_b200 import proto
     lits = [(5, T.int64), (None, T.int32), (-3, T.int8), (1.5, T.float64), (2.5, T.float32), (True, T.bool_), (1000, T.date32), (7, T.int16),
-            (decimal.Decimal("123.45"), T.decimal128(17, 2)), (None, T.null), (10**15, T.timestamp_us)]
+            (decimal.Decimal("123.45"), T.decimal128(17, 2)), (None, T.null), (10**15, T.timestamp_us),
+            ("abc", T.utf8), ("", T.utf8), (None, T.utf8), ("h\u00e9\u20ac\U0001F600" * 9, T.utf8)]
     for i, (v, dt) in enumerate(lits):
         open(os.path.join(out, "lit%d.bin" % i), "wb").write(proto.literal_ipc_bytes(v, dt))
