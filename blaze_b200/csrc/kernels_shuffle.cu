@@ -333,6 +333,313 @@ __global__ void __launch_bounds__(ENC_NT, 2) shuffle_encode_kernel(const ShufSpe
   }
 }
 
+// ---- batches with Binary columns ----------------------------------------------------------------------------------------------
+// Two-pass: the data bytes of the chunk are summed first (the host sizes the buffer and the rows per record from them), then the
+// rows get their sorted positions ONCE (perm), and every later pass — lengths, their 64-bit scans, record sizes, headers, planes,
+// bytes — reads the same positions, so the order of the length planes and of the data always agree.
+
+__device__ __forceinline__ bool vl_valid(const ShufCol& col, unsigned long long row) {
+  if (!col.validity) return true;
+  const unsigned long long bi = row + col.bit_offset;
+  return (col.validity[bi >> 3] >> (bi & 7)) & 1;
+}
+
+__device__ __forceinline__ unsigned long long vl_bytes(const ShufVarlen& vl, int k, unsigned long long q0, unsigned long long m) {
+  const unsigned long long* d = vl.doff + (unsigned long long)k * (unsigned long long)(vl.n + 1);
+  return d[q0 + m] - d[q0];
+}
+
+// largest p with a[p] <= x (a ascending, a[0] <= x < a[P])
+__device__ __forceinline__ int vl_find(const unsigned long long* a, int P, unsigned long long x) {
+  int lo = 0, hi = P;
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (a[mid] <= x) lo = mid; else hi = mid; }
+  return lo;
+}
+
+// the record holding sorted position q: its index g, first position q0, rows m, and q's row j inside it
+struct VlLoc { unsigned long long g, q0, m, j; };
+__device__ __forceinline__ VlLoc vl_locate(const ShufVarlen& vl, const unsigned long long* s_rows, int P, const unsigned long long* counts, unsigned long long q) {
+  const int p = vl_find(s_rows, P, q);
+  const unsigned long long idx = q - s_rows[p], r = idx / vl.B, t = counts[p];
+  VlLoc l;
+  l.j = idx - r * vl.B; l.q0 = s_rows[p] + r * vl.B; l.g = vl.rec_start[p] + r;
+  l.m = t - r * vl.B < vl.B ? t - r * vl.B : vl.B;
+  return l;
+}
+
+__global__ void __launch_bounds__(256) shuffle_vl_bytes_kernel(const ShufSpec sp, const ShufVarlen vl, unsigned long long* totals) {
+  const unsigned lane = threadIdx.x & 31;
+  for (int k = 0; k < vl.nb; k++) {
+    const ShufCol& col = sp.col[vl.col[k]];
+    const int32_t* __restrict__ off = vl.offsets[k];
+    unsigned long long sum = 0;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < vl.n; i += (long long)gridDim.x * blockDim.x)
+      if (vl_valid(col, (unsigned long long)i)) sum += (unsigned long long)(off[i + 1] - off[i]);
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, d);
+    if (lane == 0 && sum) atomicAdd(totals + k, sum);
+  }
+}
+
+// sorted positions: a CTA ranks a 4096-row tile per partition in shared memory and reserves the tile's rows of every partition with
+// one global atomic per (tile, partition), as shuffle_encode_kernel does; perm[row_start[p] + reserved + rank] = row
+constexpr int VR_NT = 512, VR_RPT = SHUF_TILE / VR_NT;
+__global__ void __launch_bounds__(VR_NT) shuffle_vl_rank_kernel(const ShufVarlen vl, int P, const uint16_t* __restrict__ pids, unsigned long long* cursors) {
+  __shared__ unsigned s_cnt[SHUF_MAX_PARTS], s_base[SHUF_MAX_PARTS];
+  const long long ntiles = (vl.n + SHUF_TILE - 1) / SHUF_TILE;
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const long long t0 = tile * SHUF_TILE;
+    for (int p = threadIdx.x; p < P; p += VR_NT) s_cnt[p] = 0;
+    __syncthreads();
+    unsigned pid[VR_RPT], rank[VR_RPT];
+#pragma unroll
+    for (int k = 0; k < VR_RPT; k++) {
+      const long long i = t0 + k * VR_NT + threadIdx.x;
+      pid[k] = 0; rank[k] = 0;
+      if (i < vl.n) { pid[k] = pids[i]; rank[k] = atomicAdd(&s_cnt[pid[k]], 1u); }
+    }
+    __syncthreads();
+    for (int p = threadIdx.x; p < P; p += VR_NT) {
+      const unsigned c = s_cnt[p];
+      if (c) s_base[p] = (unsigned)(vl.row_start[p] + atomicAdd(cursors + p, (unsigned long long)c));
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < VR_RPT; k++) {
+      const long long i = t0 + k * VR_NT + threadIdx.x;
+      if (i < vl.n) vl.perm[s_base[pid[k]] + rank[k]] = (uint32_t)i;
+    }
+    __syncthreads();
+  }
+}
+
+// lens[k * n + q] = data bytes of sorted position q in Binary column k (0 for NULL)
+__global__ void __launch_bounds__(256) shuffle_vl_lengths_kernel(const ShufSpec sp, const ShufVarlen vl) {
+  for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < vl.n; q += (long long)gridDim.x * blockDim.x) {
+    const unsigned long long row = vl.perm ? vl.perm[q] : (unsigned long long)q;
+    for (int k = 0; k < vl.nb; k++) {
+      const int32_t* __restrict__ off = vl.offsets[k];
+      vl.lens[(unsigned long long)k * vl.n + q] = vl_valid(sp.col[vl.col[k]], row) ? (uint32_t)(off[row + 1] - off[row]) : 0u;
+    }
+  }
+}
+
+// 64-bit exclusive scan (n -> n + 1 entries): block sums, one CTA scans the sums, final pass
+constexpr int VS_BLOCK = 256, VS_ITEMS = 8, VS_TILE = VS_BLOCK * VS_ITEMS;
+
+__device__ __forceinline__ unsigned long long vs_block_exclusive(unsigned long long v, unsigned long long* total, unsigned long long* smem /* 9 */) {
+  const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned long long incl = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) { const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += t; }
+  if (lane == 31) smem[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    const unsigned long long w = lane < VS_BLOCK / 32 ? smem[lane] : 0;
+    unsigned long long wi = w;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const unsigned long long t = __shfl_up_sync(0xffffffffu, wi, d); if (lane >= d) wi += t; }
+    if (lane < VS_BLOCK / 32) smem[lane] = wi - w;
+    if (lane == VS_BLOCK / 32 - 1) smem[8] = wi;
+  }
+  __syncthreads();
+  const unsigned long long res = incl - v + smem[warp];
+  *total = smem[8];
+  __syncthreads();
+  return res;
+}
+
+template <class T>
+__global__ void __launch_bounds__(VS_BLOCK) vl_scan_sums_kernel(const T* __restrict__ in, long long n, unsigned long long* __restrict__ sums) {
+  __shared__ unsigned long long smem[9];
+  const long long base = blockIdx.x * (long long)VS_TILE;
+  unsigned long long s = 0;
+  for (int k = 0; k < VS_ITEMS; k++) { const long long i = base + k * VS_BLOCK + threadIdx.x; if (i < n) s += in[i]; }
+  unsigned long long total; vs_block_exclusive(s, &total, smem);
+  if (threadIdx.x == 0) sums[blockIdx.x] = total;
+}
+__global__ void __launch_bounds__(VS_BLOCK) vl_scan_carry_kernel(unsigned long long* sums, long long nb) {
+  __shared__ unsigned long long smem[9];
+  unsigned long long carry = 0;
+  for (long long base = 0; base < nb; base += VS_BLOCK) {
+    const long long i = base + threadIdx.x;
+    const unsigned long long v = i < nb ? sums[i] : 0;
+    unsigned long long total; const unsigned long long ex = vs_block_exclusive(v, &total, smem);
+    if (i < nb) sums[i] = carry + ex;
+    carry += total;
+  }
+}
+template <class T>
+__global__ void __launch_bounds__(VS_BLOCK) vl_scan_final_kernel(const T* __restrict__ in, unsigned long long* __restrict__ out, long long n, const unsigned long long* __restrict__ sums) {
+  __shared__ unsigned long long smem[9];
+  const long long base = blockIdx.x * (long long)VS_TILE + (long long)threadIdx.x * VS_ITEMS;
+  unsigned long long v[VS_ITEMS], s = 0;
+#pragma unroll
+  for (int k = 0; k < VS_ITEMS; k++) { v[k] = base + k < n ? (unsigned long long)in[base + k] : 0; s += v[k]; }
+  unsigned long long total; unsigned long long ex = vs_block_exclusive(s, &total, smem) + sums[blockIdx.x];
+#pragma unroll
+  for (int k = 0; k < VS_ITEMS; k++) { if (base + k < n) out[base + k] = ex; ex += v[k]; }
+  if (base <= n - 1 && n - 1 < base + VS_ITEMS) out[n] = ex;                   // the grand total, from the owner of index n - 1
+}
+
+template <class T>
+int vl_scan(const T* in, unsigned long long* out, int64_t n, unsigned long long* sums, cudaStream_t s) {
+  const int64_t nb = (n + VS_TILE - 1) / VS_TILE;
+  vl_scan_sums_kernel<T><<<(unsigned)nb, VS_BLOCK, 0, s>>>(in, n, sums);
+  vl_scan_carry_kernel<<<1, VS_BLOCK, 0, s>>>(sums, nb);
+  vl_scan_final_kernel<T><<<(unsigned)nb, VS_BLOCK, 0, s>>>(in, out, n, sums);
+  return 3;
+}
+
+// encoded bytes of every record; err bit 0 when the Binary data of one record would exceed INT32_MAX bytes (the reader's 32-bit offsets)
+__global__ void __launch_bounds__(256) shuffle_vl_records_kernel(const ShufSpec sp, const ShufVarlen vl, int P, const unsigned long long* __restrict__ counts) {
+  for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < vl.R; g += (long long)gridDim.x * blockDim.x) {
+    const int p = vl_find(vl.rec_start, P, (unsigned long long)g);
+    const unsigned long long r = (unsigned long long)g - vl.rec_start[p], t = counts[p];
+    const unsigned long long m = t - r * vl.B < vl.B ? t - r * vl.B : vl.B, q0 = vl.row_start[p] + r * vl.B;
+    unsigned long long data = 0;
+    for (int k = 0; k < vl.nb; k++) data += vl_bytes(vl, k, q0, m);
+    vl.rec_size[g] = shuf_record_bytes(sp, m) + data;
+    if (data > 0x7FFFFFFFull) atomicOr(vl.err, 1u);
+  }
+}
+
+// varint(m) + the `has null buffer` byte of every column of every record; part_off[p] = rec_off[rec_start[p]]
+__global__ void __launch_bounds__(256) shuffle_vl_headers_kernel(const ShufSpec sp, const ShufVarlen vl, int P, const unsigned long long* __restrict__ counts,
+                                                                 unsigned long long* part_off, uint8_t* out) {
+  for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < vl.R || g <= P; g += (long long)gridDim.x * blockDim.x) {
+    if (g <= P) part_off[g] = vl.rec_off[vl.rec_start[g]];
+    if (g >= vl.R) continue;
+    const int p = vl_find(vl.rec_start, P, (unsigned long long)g);
+    const unsigned long long r = (unsigned long long)g - vl.rec_start[p], t = counts[p];
+    const unsigned long long m = t - r * vl.B < vl.B ? t - r * vl.B : vl.B, m8 = (m + 7) >> 3, q0 = vl.row_start[p] + r * vl.B;
+    uint8_t* base = out + vl.rec_off[g];
+    unsigned long long v = m; uint32_t vlen = 0;
+    while (v >= 128) { base[vlen++] = (uint8_t)(128 + (v & 127)); v >>= 7; }
+    base[vlen++] = (uint8_t)v;
+    unsigned long long before = 0; int k = 0;
+    for (int c = 0; c < sp.ncols; c++) {
+      base[col_offset(sp, c, m, m8, vlen) + before] = sp.col[c].nullable ? 1 : 0;
+      if (sp.col[c].varlen) before += vl_bytes(vl, k++, q0, m);
+    }
+  }
+}
+
+// one thread per sorted position: validity and Boolean bits, the byte planes of the fixed-width columns and the length planes.
+// Neighbouring positions are neighbouring bytes of every plane; the input rows are gathered through perm.
+constexpr int VE_NT = 256;
+__global__ void __launch_bounds__(VE_NT) shuffle_vl_encode_kernel(const ShufSpec sp, const ShufVarlen vl, int P, const unsigned long long* __restrict__ counts, uint8_t* out) {
+  __shared__ unsigned long long s_rows[SHUF_MAX_PARTS + 1];
+  for (int p = threadIdx.x; p <= P; p += VE_NT) s_rows[p] = vl.row_start[p];
+  __syncthreads();
+  for (long long q = blockIdx.x * (long long)VE_NT + threadIdx.x; q < vl.n; q += (long long)gridDim.x * VE_NT) {
+    const VlLoc l = vl_locate(vl, s_rows, P, counts, (unsigned long long)q);
+    const unsigned long long row = vl.perm ? vl.perm[q] : (unsigned long long)q, m8 = (l.m + 7) >> 3;
+    const uint32_t vlen = shuf_varint_len(l.m);
+    const unsigned long long rb = vl.rec_off[l.g];
+    unsigned long long before = 0; int k = 0;
+    for (int c = 0; c < sp.ncols; c++) {
+      const ShufCol& col = sp.col[c];
+      unsigned long long a = rb + col_offset(sp, c, l.m, m8, vlen) + before + 1;          // past the `has null buffer` byte
+      const bool valid = vl_valid(col, row);
+      if (col.nullable) { if (valid) or_bit(out, a + (l.j >> 3), (unsigned)(l.j & 7)); a += m8; }
+      if (col.width == 0) {
+        const unsigned long long bi = row + col.bit_offset;
+        if ((((const uint8_t*)col.values)[bi >> 3] >> (bi & 7)) & 1) or_bit(out, a + (l.j >> 3), (unsigned)(l.j & 7));
+        continue;
+      }
+      uint8_t* d = out + a + l.j;
+      if (col.varlen) {
+        const int32_t* __restrict__ off = vl.offsets[k];
+        const uint32_t len = valid ? (uint32_t)(off[row + 1] - off[row]) : 0u;
+#pragma unroll
+        for (int b = 0; b < 4; b++) d[(unsigned long long)b * l.m] = (uint8_t)(len >> (8 * b));
+        before += vl_bytes(vl, k++, l.q0, l.m);
+        continue;
+      }
+      unsigned long long lo = 0, hi = 0;
+      switch (col.width) {
+        case 1: lo = ((const uint8_t*)col.values)[row]; break;
+        case 2: lo = ((const uint16_t*)col.values)[row]; break;
+        case 4: lo = ((const uint32_t*)col.values)[row]; break;
+        case 8: lo = ((const unsigned long long*)col.values)[row]; break;
+        default: lo = ((const unsigned long long*)col.values)[2 * row]; hi = ((const unsigned long long*)col.values)[2 * row + 1]; break;
+      }
+      for (int b = 0; b < (int)col.width; b++) d[(unsigned long long)b * l.m] = (uint8_t)((b < 8 ? lo : hi) >> (8 * (b & 7)));
+    }
+  }
+}
+
+struct alignas(16) VlV16 { unsigned long long lo, hi; };
+
+// 16 output bytes from a source `mis` (1..15) bytes past a 16-byte boundary: two aligned loads, each output word a funnel shift
+__device__ __forceinline__ VlV16 vl_shifted16(const VlV16* __restrict__ src, int v, unsigned mis) {
+  const VlV16 a = src[v], b = src[v + 1];
+  const uint32_t w[8] = {(uint32_t)a.lo, (uint32_t)(a.lo >> 32), (uint32_t)a.hi, (uint32_t)(a.hi >> 32),
+                         (uint32_t)b.lo, (uint32_t)(b.lo >> 32), (uint32_t)b.hi, (uint32_t)(b.hi >> 32)};
+  const unsigned q = mis >> 2, sh = (mis & 3) * 8;
+  uint32_t x[5];
+#pragma unroll
+  for (int i = 0; i < 5; i++) x[i] = q == 0 ? w[i] : q == 1 ? w[i + 1] : q == 2 ? w[i + 2] : w[i + 3];
+  uint32_t o[4];
+#pragma unroll
+  for (int i = 0; i < 4; i++) o[i] = (uint32_t)(((((uint64_t)x[i + 1]) << 32) | x[i]) >> sh);
+  VlV16 r; r.lo = o[0] | ((unsigned long long)o[1] << 32); r.hi = o[2] | ((unsigned long long)o[3] << 32);
+  return r;
+}
+
+// the Binary bytes: one warp per 32 consecutive sorted positions, which it copies one after the other with all 32 lanes, so a long
+// value spreads over the warp.  Values of 64 bytes or more go as aligned 16-byte vectors (loads funnel-shifted into place when source
+// and destination disagree modulo 16), as varlen_copy_kernel does; heads and tails are byte copies.
+__global__ void __launch_bounds__(VE_NT) shuffle_vl_copy_kernel(const ShufSpec sp, const ShufVarlen vl, int P, const unsigned long long* __restrict__ counts, uint8_t* out) {
+  __shared__ unsigned long long s_rows[SHUF_MAX_PARTS + 1];
+  for (int p = threadIdx.x; p <= P; p += VE_NT) s_rows[p] = vl.row_start[p];
+  __syncthreads();
+  const unsigned lane = threadIdx.x & 31;
+  const long long warps = ((long long)gridDim.x * VE_NT) >> 5;
+  for (long long base = ((blockIdx.x * (long long)VE_NT + threadIdx.x) >> 5) * 32; base < vl.n; base += warps * 32) {
+    const long long q = base + lane;
+    VlLoc l{0, 0, 0, 0};
+    unsigned long long row = 0, rb = 0, m8 = 0; uint32_t vlen = 0;
+    if (q < vl.n) {
+      l = vl_locate(vl, s_rows, P, counts, (unsigned long long)q);
+      row = vl.perm ? vl.perm[q] : (unsigned long long)q; rb = vl.rec_off[l.g]; m8 = (l.m + 7) >> 3; vlen = shuf_varint_len(l.m);
+    }
+    const int cnt = (int)(vl.n - base < 32 ? vl.n - base : 32);
+    unsigned long long before = 0;
+    for (int k = 0; k < vl.nb; k++) {
+      const int c = vl.col[k];
+      const ShufCol& col = sp.col[c];
+      long long s0 = 0; unsigned long long d0 = 0; int len = 0;
+      if (q < vl.n) {
+        const unsigned long long* dk = vl.doff + (unsigned long long)k * (unsigned long long)(vl.n + 1);
+        s0 = vl.offsets[k][row];
+        len = (int)vl.lens[(unsigned long long)k * vl.n + q];
+        d0 = rb + col_offset(sp, c, l.m, m8, vlen) + before + 1 + (col.nullable ? m8 : 0) + 4 * l.m + (dk[q] - dk[l.q0]);
+        before += vl_bytes(vl, k, l.q0, l.m);
+      }
+      const uint8_t* data = (const uint8_t*)col.values;
+      for (int i = 0; i < cnt; i++) {
+        const uint8_t* sp8 = data + __shfl_sync(0xffffffffu, s0, i);
+        uint8_t* dp = out + __shfl_sync(0xffffffffu, d0, i);
+        const int n = __shfl_sync(0xffffffffu, len, i);
+        int done = 0;
+        if (n >= 64) {
+          const int head = (int)((16 - ((uintptr_t)dp & 15)) & 15);
+          if ((int)lane < head) dp[lane] = sp8[lane];
+          const int nv = (n - head) >> 4;
+          const uint8_t* s = sp8 + head; VlV16* vd = (VlV16*)(dp + head);
+          const unsigned mis = (unsigned)((uintptr_t)s & 15);
+          if (mis == 0) { const VlV16* vs = (const VlV16*)s; for (int v = (int)lane; v < nv; v += 32) vd[v] = vs[v]; }
+          else { const VlV16* vs = (const VlV16*)(s - mis); for (int v = (int)lane; v < nv; v += 32) vd[v] = vl_shifted16(vs, v, mis); }
+          done = head + (nv << 4);
+        }
+        for (int b = done + (int)lane; b < n; b += 32) dp[b] = sp8[b];
+      }
+    }
+  }
+}
+
 }  // namespace
 
 int launch_shuffle_pids(const ShufSpec& sp, int64_t n, uint16_t* d_pids, unsigned long long* d_counts, cudaStream_t s) {
@@ -375,6 +682,40 @@ int launch_shuffle_encode(const ShufSpec& sp, const uint16_t* d_pids, int64_t n,
   if (tma) { shuffle_encode_kernel<true><<<grid, ENC_NT, smem, s>>>(spx, d_pids, n, d_counts, d_part_off, d_cursors, d_out); return 1; }
 #endif
   shuffle_encode_kernel<false><<<grid, ENC_NT, smem, s>>>(spx, d_pids, n, d_counts, d_part_off, d_cursors, d_out);
+  return 1;
+}
+
+int64_t shuffle_varlen_scan_blocks(int64_t n) { return (n + VS_TILE - 1) / VS_TILE; }
+
+static int vl_grid(int64_t items, int per_sm) {
+  return (int)std::max<int64_t>(1, std::min<int64_t>((items + 255) / 256, (int64_t)sm_count() * per_sm));
+}
+
+int launch_shuffle_varlen_encode(const ShufSpec& sp, const ShufVarlen& vl, const uint16_t* d_pids, const unsigned long long* d_counts,
+                                 unsigned long long* d_cursors, unsigned long long* d_part_off, uint8_t* d_out, cudaStream_t s) {
+  const int P = sp.num_partitions;
+  int launches = 0;
+  if (vl.perm) {
+    cudaMemsetAsync(d_cursors, 0, (size_t)P * 8, s);
+    const int64_t ntiles = (vl.n + SHUF_TILE - 1) / SHUF_TILE;
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ntiles, (int64_t)sm_count() * 2));
+    shuffle_vl_rank_kernel<<<grid, VR_NT, 0, s>>>(vl, P, d_pids, d_cursors);
+    launches++;
+  }
+  shuffle_vl_lengths_kernel<<<vl_grid(vl.n, 8), 256, 0, s>>>(sp, vl); launches++;
+  for (int k = 0; k < vl.nb; k++) launches += vl_scan(vl.lens + (size_t)k * (size_t)vl.n, vl.doff + (size_t)k * (size_t)(vl.n + 1), vl.n, vl.sums, s);
+  shuffle_vl_records_kernel<<<vl_grid(vl.R, 8), 256, 0, s>>>(sp, vl, P, d_counts); launches++;
+  launches += vl_scan(vl.rec_size, vl.rec_off, vl.R, vl.sums, s);
+  const int hgrid = vl_grid(std::max<int64_t>(vl.R, P + 1), 8);
+  shuffle_vl_headers_kernel<<<hgrid, 256, 0, s>>>(sp, vl, P, d_counts, d_part_off, d_out); launches++;
+  shuffle_vl_encode_kernel<<<vl_grid(vl.n, 8), VE_NT, 0, s>>>(sp, vl, P, d_counts, d_out); launches++;
+  shuffle_vl_copy_kernel<<<vl_grid(vl.n, 8), VE_NT, 0, s>>>(sp, vl, P, d_counts, d_out); launches++;
+  return launches;
+}
+
+int launch_shuffle_varlen_bytes(const ShufSpec& sp, const ShufVarlen& vl, unsigned long long* d_totals, cudaStream_t s) {
+  if (vl.n <= 0 || vl.nb == 0) return 0;
+  shuffle_vl_bytes_kernel<<<vl_grid(vl.n, 8), 256, 0, s>>>(sp, vl, d_totals);
   return 1;
 }
 

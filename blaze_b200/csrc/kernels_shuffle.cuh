@@ -21,7 +21,7 @@ struct ShufCol {
   uint8_t width;                            // 0: Boolean (bits), else 1, 2, 4, 8, 16 bytes
   uint8_t nullable;                         // the field is nullable: the record carries a validity bitmap for it
   uint8_t tma;                              // set by the launcher: the column's tiles are staged by cp.async.bulk (16-byte aligned, width 1/2/4/8)
-  uint8_t _pad[1];
+  uint8_t varlen;                           // Binary: width 4 (the int32 length planes), `values` = the data base the offsets index
   uint32_t k8, kw;                          // columns before this one take k8 * ceil(m/8) + kw * m bytes (+ one flag byte each)
 };
 
@@ -51,5 +51,35 @@ int launch_shuffle_layout(const ShufSpec& sp, const unsigned long long* d_counts
 // scatter + encode: every value lands in its byte planes
 int launch_shuffle_encode(const ShufSpec& sp, const uint16_t* d_pids, int64_t n, const unsigned long long* d_counts, const unsigned long long* d_part_off,
                           unsigned long long* d_cursors, uint8_t* d_out, cudaStream_t s);
+
+// ---- batches with Binary columns (batch_serde.rs:595-619 + write_offsets :217-240): after the `has null buffer` byte and the
+// validity bytes, a Binary column of a record of m rows is its m int32 lengths as 4 byte planes (a NULL row has length 0), then
+// the bytes of its rows in row order.  A record's size now depends on the data, so the layout is computed in passes over
+// positions assigned once: sorted position q of the chunk = partition-major order, row perm[q] of the input.
+constexpr int SHUF_MAX_VARLEN = SHUF_MAX_COLS;
+struct ShufVarlen {
+  int32_t nb;                               // Binary columns
+  uint32_t B;                               // rows per record (the last record of a partition holds the rest)
+  long long n, R;                           // rows and records of the chunk
+  int8_t col[SHUF_MAX_VARLEN];              // column index of the k-th Binary column, ascending
+  const int32_t* offsets[SHUF_MAX_VARLEN];  // its Arrow offsets, advanced by the Arrow offset (offsets[0] may be > 0)
+  // device work arrays of the chunk
+  uint32_t* perm;                           // n: sorted position -> input row (null when P = 1: the identity)
+  uint32_t* lens;                           // nb * n: data bytes of every sorted position per Binary column
+  unsigned long long* doff;                 // nb * (n + 1): exclusive prefix of `lens` (64-bit: a chunk may carry > 4 GiB)
+  const unsigned long long* row_start;      // P + 1: first sorted position of every partition
+  const unsigned long long* rec_start;      // P + 1: first record of every partition
+  unsigned long long* rec_size;             // R: encoded bytes of every record
+  unsigned long long* rec_off;              // R + 1: byte offset of every record in the chunk's buffer
+  unsigned long long* sums;                 // scan block sums: shuffle_varlen_scan_blocks(max(n, R)) entries
+  unsigned* err;                            // bit 0: one record holds more than INT32_MAX bytes of Binary data
+};
+int64_t shuffle_varlen_scan_blocks(int64_t n);
+// totals[k] += data bytes of the non-NULL rows of Binary column k (input order; totals zeroed)
+int launch_shuffle_varlen_bytes(const ShufSpec& sp, const ShufVarlen& vl, unsigned long long* d_totals, cudaStream_t s);
+// with row_start / rec_start uploaded and d_out zeroed where bits are OR-ed in: ranks the rows (P > 1), scans the lengths, sizes and
+// places the records (part_off, P + 1 entries), writes headers, fixed-width planes, length planes and the Binary bytes
+int launch_shuffle_varlen_encode(const ShufSpec& sp, const ShufVarlen& vl, const uint16_t* d_pids, const unsigned long long* d_counts,
+                                 unsigned long long* d_cursors, unsigned long long* d_part_off, uint8_t* d_out, cudaStream_t s);
 
 }  // namespace b200q

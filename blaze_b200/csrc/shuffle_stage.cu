@@ -11,9 +11,13 @@
 // frames them per partition into compression blocks (host threads, lz4_frame.cc) and writes the two files exactly as
 // the no-spill branch of shuffle_write does.  A partition of the file = the blocks of chunk 0, chunk 1, ... for it —
 // the same shape the reference produces when it merges spills (sort_repartitioner.rs:226-246).
+// Binary columns (the frozen accumulator rows AggExec(Partial) emits in the reference format) are encoded too: such a chunk sums
+// its data bytes first, then cuts records of compute_suggested_batch_size_for_output rows and brings back every record's offset,
+// so the compression blocks end on record boundaries (kernels_shuffle.cu, "batches with Binary columns").
 // Not on the GPU path (B200Q_ERR_UNSUPPORTED -> the host keeps its CPU operator, INTEGRATION.md §3): range and
-// round-robin partitioning (they need the sort operator first, shuffle_writer_exec.rs:133-158), Binary / nested columns,
-// more than 4096 partitions, codec zstd.
+// round-robin partitioning (they need the sort operator first, shuffle_writer_exec.rs:133-158), Utf8 / Null / nested columns,
+// Binary hash keys, more than 4096 partitions, codec zstd.
+#include <algorithm>
 #include <atomic>
 #include <cstdio>
 #include <cstring>
@@ -30,6 +34,7 @@ namespace {
 struct ShuffleChunk {
   int64_t rows = 0;
   std::vector<unsigned long long> part_off, part_rows;      // host copies: P + 1 byte offsets, P row counts
+  std::vector<unsigned long long> rec_start, rec_off;       // chunks with Binary columns: first record of each partition (P + 1), record offsets (R + 1)
   std::vector<uint8_t> host;                                // encoded bytes (shuffle_output_to_host)
   DevMemP dev;                                              // encoded bytes in HBM (kept when the result stays on the device)
 };
@@ -39,6 +44,7 @@ class ShuffleWriteStage : public Stage, public ShuffleResult {
   std::vector<int> hash_cols_;
   int P_ = 1;
   bool any_bits_ = false;
+  std::vector<int> varlen_cols_;                            // Binary columns, ascending
   std::string data_file_, index_file_;
   std::vector<ShuffleChunk> chunks_;
   std::vector<uint64_t> file_offsets_;
@@ -59,9 +65,12 @@ class ShuffleWriteStage : public Stage, public ShuffleResult {
     uint32_t k8 = 0, kw = 0;
     for (size_t i = 0; i < in.fields.size(); i++) {
       const FieldDef& f = in.fields[i];
-      if (f.type.is_varlen() || f.type.id == T_NULL) throw PlanError(B200Q_ERR_UNSUPPORTED, "shuffle of a " + f.type.str() + " column is not on the GPU path");
+      const bool binary = f.type.id == T_BINARY;
+      if ((f.type.is_varlen() && !binary) || f.type.id == T_NULL) throw PlanError(B200Q_ERR_UNSUPPORTED, "shuffle of a " + f.type.str() + " column is not on the GPU path");
       ShufCol& c = base_.col[i];
-      c.width = (uint8_t)f.type.byte_width(); c.nullable = f.nullable ? 1 : 0; c.k8 = k8; c.kw = kw;
+      c.width = binary ? 4 : (uint8_t)f.type.byte_width(); c.nullable = f.nullable ? 1 : 0; c.k8 = k8; c.kw = kw;      // Binary: its int32 length planes
+      c.varlen = binary ? 1 : 0;
+      if (binary) varlen_cols_.push_back((int)i);
       if (c.nullable) k8++;
       if (c.width == 0) k8++; else kw += c.width;
       any_bits_ = any_bits_ || c.nullable || c.width == 0;
@@ -73,6 +82,7 @@ class ShuffleWriteStage : public Stage, public ShuffleResult {
       if (node.hash_exprs.size() > 8) throw PlanError(B200Q_ERR_UNSUPPORTED, "more than 8 hash partitioning expressions");
       for (auto& e : node.hash_exprs) {
         if (e->kind != E_COLUMN) throw PlanError(B200Q_ERR_UNSUPPORTED, "hash partitioning on a computed expression (project it first)");
+        if (e->type.is_varlen()) throw PlanError(B200Q_ERR_UNSUPPORTED, "hash partitioning on a " + e->type.str() + " column (murmur3 over bytes) is not on the GPU path");
         base_.key_col[base_.nkeys] = (int8_t)e->col_index; base_.key_phys[base_.nkeys] = (uint8_t)phys_of(e->type); base_.nkeys++;
       }
     }
@@ -85,6 +95,7 @@ class ShuffleWriteStage : public Stage, public ShuffleResult {
   }
 
   void encode_chunk(OpContext& cx, DevBatch& in, int64_t r0, int64_t n) {
+    if (!varlen_cols_.empty()) { encode_chunk_varlen(cx, in, r0, n); return; }
     ShufSpec sp = base_;
     for (int i = 0; i < sp.ncols; i++) {
       const DevColumn& dc = in.cols[i]; ShufCol& c = sp.col[i];
@@ -131,26 +142,147 @@ class ShuffleWriteStage : public Stage, public ShuffleResult {
     chunks_.push_back(std::move(ch));
   }
 
+  // rows per record of a chunk with Binary columns: compute_suggested_batch_size_for_output (datafusion-ext-commons/src/lib.rs:93-116)
+  // over the chunk's Arrow buffer bytes (get_batch_mem_size: offsets, data, values, validity)
+  int64_t varlen_batch_size(int64_t n, unsigned long long data_bytes) const {
+    unsigned long long mem = data_bytes;
+    for (int c = 0; c < base_.ncols; c++) {
+      const ShufCol& col = base_.col[c];
+      mem += col.varlen ? 4ull * (unsigned long long)(n + 1) : col.width ? (unsigned long long)col.width * (unsigned long long)n : (unsigned long long)(n + 7) / 8;
+      mem += (unsigned long long)(n + 7) / 8;
+    }
+    const unsigned long long per_row = std::max<unsigned long long>(mem, 16) / (unsigned long long)std::max<int64_t>(n, 1);
+    const unsigned long long sub = (8ull << 20) / std::max<unsigned long long>(per_row, 16);
+    return (int64_t)std::max<unsigned long long>(20, std::min<unsigned long long>(sub, (unsigned long long)base_.batch_size));
+  }
+
+  // Binary columns: the record sizes depend on the data.  Pass 1 sums the data bytes (brought back with the partition counts in one
+  // round trip); the host then fixes the rows per record, the record count and the buffer size, and the device assigns every row its
+  // sorted position once, scans the lengths in that order (64-bit), sizes and places the records and writes them.
+  void encode_chunk_varlen(OpContext& cx, DevBatch& in, int64_t r0, int64_t n) {
+    ShufSpec sp = base_;
+    ShufVarlen vl{};
+    vl.n = n; vl.nb = (int)varlen_cols_.size();
+    for (int i = 0; i < sp.ncols; i++) {
+      const DevColumn& dc = in.cols[i]; ShufCol& c = sp.col[i];
+      const int64_t off = dc.offset + r0;
+      if (off > 0xFFFFFFFFLL) throw ExecError(B200Q_ERR_UNSUPPORTED, "column offset beyond 2^32 rows");
+      if (!dc.values) throw ExecError(B200Q_ERR_INVALID_ARG, "shuffle: column without a values buffer");
+      if (dc.validity && !c.nullable) throw ExecError(B200Q_ERR_INVALID_ARG, "shuffle: validity bitmap on a column the schema declares non-nullable");
+      c.validity = dc.validity ? (const uint8_t*)dc.validity->ptr : nullptr;
+      c.bit_offset = (uint32_t)off;
+      if (c.varlen) {
+        if (!dc.offsets) throw ExecError(B200Q_ERR_INVALID_ARG, "shuffle: Binary column without an offsets buffer");
+        c.values = dc.values->ptr;                                                  // the data base the offsets index
+        const int k = (int)(std::find(varlen_cols_.begin(), varlen_cols_.end(), i) - varlen_cols_.begin());
+        vl.col[k] = (int8_t)i; vl.offsets[k] = (const int32_t*)dc.offsets->ptr + off;
+      } else {
+        c.values = c.width ? (const uint8_t*)dc.values->ptr + (size_t)off * c.width : (const uint8_t*)dc.values->ptr;
+      }
+    }
+    const size_t P1 = (size_t)P_ + 1, nb = (size_t)vl.nb;
+    unsigned long long* d_counts = (unsigned long long*)d_small_->ptr;
+    unsigned long long* d_part_off = d_counts + P_;
+    unsigned long long* d_cursors = d_part_off + P_ + 1;
+    DevMemP d_meta = DevMem::alloc((2 * P1 + nb + 1) * 8, cx.stream);           // row_start | rec_start | totals | err
+    unsigned long long* d_row_start = (unsigned long long*)d_meta->ptr;
+    unsigned long long* d_rec_start = d_row_start + P1;
+    unsigned long long* d_totals = d_rec_start + P1;
+    DevMemP d_pids = P_ > 1 ? DevMem::alloc((size_t)n * 2 + 16, cx.stream) : nullptr;
+    B200Q_CUDA(cudaEventRecord(cx.ev0, cx.stream));
+    B200Q_CUDA(cudaMemsetAsync(d_counts, 0, (size_t)P_ * 8, cx.stream));
+    B200Q_CUDA(cudaMemsetAsync(d_totals, 0, (nb + 1) * 8, cx.stream));
+    if (P_ > 1) cx.m.launches += launch_shuffle_pids(sp, n, (uint16_t*)d_pids->ptr, d_counts, cx.stream);
+    else { const unsigned long long nn = (unsigned long long)n; B200Q_CUDA(cudaMemcpyAsync(d_counts, &nn, 8, cudaMemcpyHostToDevice, cx.stream)); }
+    cx.m.launches += launch_shuffle_varlen_bytes(sp, vl, d_totals, cx.stream);
+    ShuffleChunk ch; ch.rows = n; ch.part_off.resize(P1); ch.part_rows.resize((size_t)P_);
+    std::vector<unsigned long long> totals(nb);
+    B200Q_CUDA(cudaMemcpyAsync(ch.part_rows.data(), d_counts, (size_t)P_ * 8, cudaMemcpyDeviceToHost, cx.stream));
+    B200Q_CUDA(cudaMemcpyAsync(totals.data(), d_totals, nb * 8, cudaMemcpyDeviceToHost, cx.stream));
+    B200Q_CUDA(cudaStreamSynchronize(cx.stream));
+    unsigned long long data_bytes = 0;
+    for (unsigned long long t : totals) data_bytes += t;
+    const unsigned long long B = (unsigned long long)varlen_batch_size(n, data_bytes);
+    std::vector<unsigned long long> row_start(2 * P1);                            // row_start | rec_start, uploaded together
+    unsigned long long rows = 0, R = 0;
+    for (size_t p = 0; p < (size_t)P_; p++) {
+      row_start[p] = rows; row_start[P1 + p] = R;
+      rows += ch.part_rows[p]; R += (ch.part_rows[p] + B - 1) / B;
+    }
+    row_start[(size_t)P_] = rows; row_start[P1 + (size_t)P_] = R;
+    if (rows != (unsigned long long)n) throw ExecError(B200Q_ERR_EXECUTION, "internal: shuffle partition counts do not add up to the chunk's rows");
+    ch.rec_start.assign(row_start.begin() + (ptrdiff_t)P1, row_start.end());
+    const unsigned long long cap = (unsigned long long)sp.tot_kw * (unsigned long long)n + (unsigned long long)sp.tot_k8 * ((unsigned long long)n / 8 + R) +
+                                   (unsigned long long)(5 + sp.ncols) * R + data_bytes + 64;
+    B200Q_CUDA(cudaMemcpyAsync(d_row_start, row_start.data(), 2 * P1 * 8, cudaMemcpyHostToDevice, cx.stream));
+    DevMemP d_out = DevMem::alloc((size_t)cap, cx.stream);
+    DevMemP d_perm = P_ > 1 ? DevMem::alloc((size_t)n * 4, cx.stream) : nullptr;
+    DevMemP d_lens = DevMem::alloc(nb * (size_t)n * 4, cx.stream);
+    DevMemP d_doff = DevMem::alloc(nb * (size_t)(n + 1) * 8, cx.stream);
+    DevMemP d_recs = DevMem::alloc((size_t)(2 * R + 1) * 8, cx.stream);           // rec_size | rec_off
+    DevMemP d_sums = DevMem::alloc((size_t)shuffle_varlen_scan_blocks(std::max<int64_t>(n, (int64_t)R)) * 8 + 16, cx.stream);
+    vl.B = (uint32_t)B; vl.R = (long long)R;
+    vl.perm = d_perm ? (uint32_t*)d_perm->ptr : nullptr;
+    vl.lens = (uint32_t*)d_lens->ptr; vl.doff = (unsigned long long*)d_doff->ptr;
+    vl.row_start = d_row_start; vl.rec_start = d_rec_start;
+    vl.rec_size = (unsigned long long*)d_recs->ptr; vl.rec_off = vl.rec_size + R;
+    vl.sums = (unsigned long long*)d_sums->ptr; vl.err = (unsigned*)(d_totals + nb);
+    if (any_bits_) B200Q_CUDA(cudaMemsetAsync(d_out->ptr, 0, (size_t)cap, cx.stream));      // bit regions are OR-ed into
+    cx.m.launches += launch_shuffle_varlen_encode(sp, vl, P_ > 1 ? (const uint16_t*)d_pids->ptr : nullptr, d_counts, d_cursors, d_part_off, (uint8_t*)d_out->ptr, cx.stream);
+    cx.m.fast_launches++;
+    B200Q_CUDA(cudaGetLastError());
+    B200Q_CUDA(cudaEventRecord(cx.ev1, cx.stream));
+    ch.rec_off.resize((size_t)R + 1);
+    unsigned err = 0;
+    B200Q_CUDA(cudaMemcpyAsync(ch.part_off.data(), d_part_off, P1 * 8, cudaMemcpyDeviceToHost, cx.stream));
+    B200Q_CUDA(cudaMemcpyAsync(ch.rec_off.data(), vl.rec_off, (size_t)(R + 1) * 8, cudaMemcpyDeviceToHost, cx.stream));
+    B200Q_CUDA(cudaMemcpyAsync(&err, vl.err, 4, cudaMemcpyDeviceToHost, cx.stream));
+    B200Q_CUDA(cudaStreamSynchronize(cx.stream));
+    { float ms = 0; B200Q_CUDA(cudaEventElapsedTime(&ms, cx.ev0, cx.ev1)); cx.m.gpu_ms += ms; if (cx.cur_stage == 0) { cx.m.hot_ms += ms; cx.m.hot_rows += n; cx.m.hot_launches++; } }
+    if (err & 1) throw ExecError(B200Q_ERR_UNSUPPORTED, "one shuffle record would carry more than INT32_MAX (2^31 - 1) bytes of Binary data, "
+                                                        "the limit of the reader's 32-bit offsets; push smaller batches or lower batch_size");
+    const unsigned long long total = ch.part_off[(size_t)P_];
+    if (total > cap) throw ExecError(B200Q_ERR_EXECUTION, "internal: encoded shuffle chunk larger than its bound");
+    if (cx.conf.shuffle_output_on_device) ch.dev = d_out;
+    else {
+      ch.host.resize((size_t)total);
+      if (total) B200Q_CUDA(cudaMemcpyAsync(ch.host.data(), d_out->ptr, (size_t)total, cudaMemcpyDeviceToHost, cx.stream));
+      B200Q_CUDA(cudaStreamSynchronize(cx.stream));
+      cx.m.d2h_bytes += (int64_t)total;
+    }
+    chunks_.push_back(std::move(ch));
+  }
+
   // ---- finish: frame + write (sort_repartitioner.rs:151-185, buffered_data.rs:123-158) ---------------------------------
   // one compression block = whole records of one (chunk, partition) up to ~4 MiB of payload (ipc_compression.rs:77-83 cuts
   // on 0.9 x 4 MiB of *compressed* bytes; where a block ends is not observable by a reader, :129-165)
   void compress_partition(int p, std::vector<uint8_t>& out) const {
     const unsigned long long B = (unsigned long long)base_.batch_size, F = shuf_record_bytes(base_, B);
     constexpr unsigned long long TARGET = 4ull << 20;
+    auto block = [&out](const uint8_t* src, unsigned long long blen) {
+      const size_t at = out.size();
+      out.resize(at + 4);
+      lz4_frame_append(src, (size_t)blen, out);
+      const uint32_t framed = (uint32_t)(out.size() - at - 4);
+      memcpy(out.data() + at, &framed, 4);
+    };
     for (const ShuffleChunk& ch : chunks_) {
       const unsigned long long t = ch.part_rows[(size_t)p];
       if (t == 0) continue;
+      if (!ch.rec_off.empty()) {                            // Binary columns: records differ in size, cut at the recorded boundaries
+        const unsigned long long g1 = ch.rec_start[(size_t)p + 1];
+        for (unsigned long long g = ch.rec_start[(size_t)p]; g < g1;) {
+          unsigned long long h = g + 1;                     // a record larger than the target is a block of its own
+          while (h < g1 && ch.rec_off[h + 1] - ch.rec_off[g] <= TARGET) h++;
+          block(ch.host.data() + ch.rec_off[g], ch.rec_off[h] - ch.rec_off[g]);
+          g = h;
+        }
+        continue;
+      }
       const uint8_t* src = ch.host.data() + ch.part_off[(size_t)p];
       const unsigned long long len = ch.part_off[(size_t)p + 1] - ch.part_off[(size_t)p];
       const unsigned long long per_block = std::max<unsigned long long>(1, TARGET / F) * F;     // whole records
-      for (unsigned long long pos = 0; pos < len; pos += per_block) {
-        const unsigned long long blen = std::min(per_block, len - pos);
-        const size_t at = out.size();
-        out.resize(at + 4);
-        lz4_frame_append(src + pos, (size_t)blen, out);
-        const uint32_t framed = (uint32_t)(out.size() - at - 4);
-        memcpy(out.data() + at, &framed, 4);
-      }
+      for (unsigned long long pos = 0; pos < len; pos += per_block) block(src + pos, std::min(per_block, len - pos));
     }
   }
 

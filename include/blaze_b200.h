@@ -255,7 +255,9 @@ b200q_status b200q_snappy_uncompress(const uint8_t* src, size_t n, uint8_t* dst,
 /* ---- ShuffleWriterExec result (plans rooted at ShuffleWriterExecNode) ----------------------------------------
  * Every pushed batch becomes one CHUNK: the rows of the batch grouped by output partition
  * (pmod(murmur3(hash exprs, 42), n), shuffle/mod.rs:163-188) and encoded as the reference's `batch_serde`
- * records (batch_serde.rs:66-77; records of at most conf.batch_size rows).  Bytes [part_off[p], part_off[p+1]) of
+ * records (batch_serde.rs:66-77; records of at most conf.batch_size rows).  Binary columns (the frozen accumulator rows of a
+ * reference-format AggExec(Partial)) are encoded too: a chunk that carries them cuts records at the reference's suggested batch
+ * size for its bytes (compute_suggested_batch_size_for_output, lib.rs:93-116).  Bytes [part_off[p], part_off[p+1]) of
  * `data` are partition p's records of that chunk, UNcompressed.  b200q_op_finish frames them into
  * `u32 length ‖ LZ4 frame` blocks and writes the .data / .index files (unless conf.shuffle_output_on_device).
  * Pointers stay valid until b200q_op_destroy. */

@@ -351,3 +351,56 @@ if any(t in (ONLY or "S1,S2,S3") for t in ("S1", "S2", "S3")):
         assert len(got) == groups and all(got[k] == int(want[k]) for k in got), "S3 sums differ from the torch computation"
         return 16 * len(got)
     run_strings("S3 SUM(TryCast(ns AS BIGINT)) GROUP BY k", s3, [kg, (ns_data, ns_offs)], 8 * srows + ns_offs.numel() * 4 + ns_data.numel(), s3_check)
+
+
+# B1-B2: Binary columns through ShuffleWriterExec (the reference-format AggExec(Partial) output carries one Binary column of frozen
+# accumulator rows).  Timed like S1-S3: push_device -> finish -> sync, chunks kept on the device.
+def run_shuffle_wall(name, plan, spec, keep, conf, n, alg_bytes=None):
+    if ONLY and not any(t in name for t in ONLY.split(",")): return
+    import time
+    best = None
+    for _ in range(REPS or 3):
+        with native.NativeOp(plan.plan_bytes(), conf, 0) as op:
+            torch.cuda.synchronize(); t0 = time.perf_counter()
+            op.push_device(native.DeviceBatch(spec, n, 0, keepalive=keep))
+            op.finish(); op.sync()
+            dt = time.perf_counter() - t0
+            m = op.metrics(); chunks = op.shuffle_chunks()
+        if best is None or dt < best[0]: best = (dt, m, chunks)
+    dt, m, chunks = best
+    out = {"shape": name, "rows": n, "wall_ms_push_to_sync": dt * 1e3, "rows_per_s": n / dt, "shuffle_chunk_rows": sum(sum(c["part_rows"]) for c in chunks),
+           "encoded_bytes": sum(c["part_off"][-1] for c in chunks), "hot_kernel_ms": m["hot_kernel_ns"] / 1e6, "launches": m["gpu_kernel_launches"]}
+    if alg_bytes:
+        out.update(alg_bytes=alg_bytes, alg_GBps=alg_bytes / dt / 1e9, frac_of_hbm_peak=alg_bytes / dt / 1e9 / peak)
+    print(json.dumps(out), flush=True)
+
+
+brows = int(os.environ.get("ROWS", 1 << 26))
+if any(t in (ONLY or "B1,B2") for t in ("B1", "B2")):
+    # B1: 200-way shuffle of [k int64, b Binary] with 10-14-byte values (the size of a SUM+COUNT frozen row); algorithmic bytes from
+    # the generated buffers: read 8 + 4 + data bytes, write 8 + 4 + data bytes per row
+    bk = torch.randint(-2**62, 2**62, (brows,), dtype=torch.int64, device=dev, generator=g)
+    bl = torch.randint(10, 15, (brows,), device=dev, generator=g)
+    bdata, boffs = utf8_column(bl, 0, 256)
+    b_sch = T.Schema([T.Field("k", T.int64, False), T.Field("b", T.binary, False)])
+    b1 = PL.ShuffleWriterExec(PL.MemoryExec(b_sch), ("hash", [E.Column("k")], 200), "", "")
+    run_shuffle_wall("B1 shuffle write 200-way [k int64, b Binary 10-14 B]", b1, [(bk.data_ptr(), 0, brows), (bdata.data_ptr(), 0, brows, boffs.data_ptr())],
+                     [bk, bdata, boffs], native.default_conf(shuffle_output_on_device=1), brows, alg_bytes=2 * (12 * brows + bdata.numel()))
+    del bk, bl, bdata, boffs
+    # B2: the q1 map side as Spark plans it: Filter (s = 0.2) -> AggExec(Partial, SUM + COUNT GROUP BY k1, k2) -> ShuffleWriterExec 200-way
+    # on (k1, k2); the reference-format partial state (one Binary column) against the columnar partial state of the same plan
+    bf = torch.randint(0, 1000, (brows,), dtype=torch.int64, device=dev, generator=g)
+    bk1 = torch.randint(0, 1 << 17, (brows,), dtype=torch.int64, device=dev, generator=g)
+    bk2 = torch.randint(0, 8, (brows,), dtype=torch.int64, device=dev, generator=g)
+    bv = torch.randint(-10**6, 10**6, (brows,), dtype=torch.int64, device=dev, generator=g)
+    q_sch = T.Schema([T.Field(nm, T.int64, False) for nm in ("f", "k1", "k2", "v")])
+    q_preds = [E.BinaryExpr(E.Column("f"), "GtEq", E.Literal(200, T.int64)), E.BinaryExpr(E.Column("f"), "LtEq", E.Literal(399, T.int64))]
+    q_aggs = [E.AggExpr("s", E.PARTIAL, PL.create_agg(E.AGG_SUM, [E.Column("v")], q_sch, T.int64)), E.AggExpr("c", E.PARTIAL, PL.create_agg(E.AGG_COUNT, [E.Column("v")], q_sch, T.int64))]
+    q_spec = [(t.data_ptr(), 0, brows) for t in (bf, bk1, bk2, bv)]
+    for columnar in (False, True):
+        part = PL.AggExec(PL.HashAgg, [E.GroupingExpr("k1", E.Column("k1")), E.GroupingExpr("k2", E.Column("k2"))], q_aggs, True,
+                          PL.FilterExec(q_preds, PL.MemoryExec(q_sch)), columnar_state=columnar)
+        w = PL.ShuffleWriterExec(part, ("hash", [E.Column("k1"), E.Column("k2")], 200), "", "")
+        run_shuffle_wall("B2 q1 map side: Filter -> AggExec(Partial) -> ShuffleWriterExec 200-way, " + ("columnar partial state" if columnar else "reference format (Binary state)"),
+                         w, q_spec, [bf, bk1, bk2, bv], native.default_conf(shuffle_output_on_device=1, partial_state_columnar=int(columnar), agg_initial_groups=1 << 20), brows)
+    del bf, bk1, bk2, bv
