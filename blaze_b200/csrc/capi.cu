@@ -166,6 +166,31 @@ static void build_pipeline(b200q_op* op) {
   std::vector<ExprP> cur_cols = identity_cols(stage_in), filters;
   const PlanNode* last = chain[0];
   bool pending_tail = chain.size() == 1;
+  // the aggregate chain[i] over the columns of each set (one set: `cur_cols`); on return chain[i] is the last node the stage consumed
+  auto push_agg = [&](size_t& i, const std::vector<std::vector<ExprP>>& set_cols) {
+    PlanNode* n = chain[i];
+    std::vector<AggSetExprs> sets;
+    for (auto& cols : set_cols) {
+      AggSetExprs sx;
+      for (auto& g : n->group_exprs) sx.group_exprs.push_back(substitute(g, cols));
+      for (auto& a : n->aggs) { std::vector<ExprP> v; if (a.mode == MODE_PARTIAL) for (auto& e : a.args) v.push_back(substitute(e, cols)); sx.agg_args.push_back(v); }
+      sets.push_back(std::move(sx));
+    }
+    // AggExec(Final) directly above AggExec(Partial) in the same op (Spark plans this when the child is already partitioned on the grouping keys):
+    // the Partial stage's table holds one entry per group, so a Final stage would only re-insert unique keys into a second table.  One stage
+    // accumulates from the raw inputs and emits the Final columns (AVG division, result types) straight from its table.
+    PlanNode fused;
+    const PlanNode* agg_node = n;
+    last = n;
+    if (i + 1 < chain.size() && fusable_partial_final(*n, *chain[i + 1])) {
+      fused = *n; fused.need_final_merge = true; fused.schema = chain[i + 1]->schema;
+      agg_node = &fused; last = chain[i + 1]; i++;
+    }
+    if (sets.size() > 1) op->stages.push_back(make_agg_stage(op->cx, stage_in, filters, *agg_node, sets[0].group_exprs, sets[0].agg_args, sets));
+    else op->stages.push_back(make_agg_stage(op->cx, stage_in, filters, *agg_node, sets[0].group_exprs, sets[0].agg_args));
+    stage_in = op->stages.back()->out_schema;
+    cur_cols = identity_cols(stage_in); filters.clear(); pending_tail = false;
+  };
   for (size_t i = 1; i < chain.size(); i++) {
     PlanNode* n = chain[i];
     last = n;
@@ -173,21 +198,22 @@ static void build_pipeline(b200q_op* op) {
     else if (n->kind == N_PROJECT) { std::vector<ExprP> nc; for (auto& e : n->proj_exprs) nc.push_back(substitute(e, cur_cols)); cur_cols = nc; pending_tail = true; }
     else if (n->kind == N_AGG) {
       if (n->need_partial_merge && !is_identity(cur_cols, stage_in)) throw PlanError(B200Q_ERR_UNSUPPORTED, "Projection fused below a merge-mode aggregate");
-      std::vector<ExprP> gex; for (auto& g : n->group_exprs) gex.push_back(substitute(g, cur_cols));
-      std::vector<std::vector<ExprP>> aargs;
-      for (auto& a : n->aggs) { std::vector<ExprP> v; if (a.mode == MODE_PARTIAL) for (auto& e : a.args) v.push_back(substitute(e, cur_cols)); aargs.push_back(v); }
-      // AggExec(Final) directly above AggExec(Partial) in the same op (Spark plans this when the child is already partitioned on the grouping keys):
-      // the Partial stage's table holds one entry per group, so a Final stage would only re-insert unique keys into a second table.  One stage
-      // accumulates from the raw inputs and emits the Final columns (AVG division, result types) straight from its table.
-      PlanNode fused;
-      const PlanNode* agg_node = n;
-      if (i + 1 < chain.size() && fusable_partial_final(*n, *chain[i + 1])) {
-        fused = *n; fused.need_final_merge = true; fused.schema = chain[i + 1]->schema;
-        agg_node = &fused; last = chain[i + 1]; i++;
-      }
-      op->stages.push_back(make_agg_stage(op->cx, stage_in, filters, *agg_node, gex, aargs));
-      stage_in = op->stages.back()->out_schema;
-      cur_cols = identity_cols(stage_in); filters.clear(); pending_tail = false;
+      push_agg(i, {cur_cols});
+    } else if (n->kind == N_EXPAND) {
+      std::vector<std::vector<ExprP>> sets;
+      for (auto& proj : n->expand_projections) { std::vector<ExprP> v; for (auto& e : proj) v.push_back(substitute(e, cur_cols)); sets.push_back(v); }
+      if (sets.size() == 1) { cur_cols = sets[0]; pending_tail = true; continue; }       // one projection: a ProjectExec
+      // Expand -> [Project]* -> AggExec(Partial): the sets are fused into the aggregate (each input row is read once and inserted once per
+      // set; filters below the Expand are shared by all sets).  Anything else above the Expand sees it materialised.
+      std::vector<std::vector<ExprP>> composed = sets;
+      size_t j = i + 1;
+      for (; j < chain.size() && chain[j]->kind == N_PROJECT; j++)
+        for (auto& cols : composed) { std::vector<ExprP> nc; for (auto& e : chain[j]->proj_exprs) nc.push_back(substitute(e, cols)); cols = nc; }
+      bool fuse = sets.size() > 1 && j < chain.size() && chain[j]->kind == N_AGG && !chain[j]->need_partial_merge;
+      if (fuse) for (auto& a : chain[j]->aggs) fuse = fuse && a.mode == MODE_PARTIAL;
+      if (fuse) { i = j; push_agg(i, composed); continue; }
+      op->stages.push_back(make_expand_stage(op->cx, stage_in, filters, sets, n->schema));
+      stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in); filters.clear(); pending_tail = false;
     } else if (n->kind == N_SORT) {
       if (pending_tail) {
         op->stages.push_back(make_filter_project_stage(op->cx, stage_in, filters, cur_cols, n->input->schema));

@@ -102,7 +102,7 @@ struct AggDef {
   }
 };
 
-enum NodeKind : uint8_t { N_LEAF, N_FILTER, N_PROJECT, N_AGG, N_SHUFFLE_WRITER, N_JOIN_BUILD, N_JOIN, N_SORT };
+enum NodeKind : uint8_t { N_LEAF, N_FILTER, N_PROJECT, N_AGG, N_SHUFFLE_WRITER, N_JOIN_BUILD, N_JOIN, N_SORT, N_EXPAND };
 enum ShuffleKind : uint8_t { SHUFFLE_SINGLE = 0, SHUFFLE_HASH = 1, SHUFFLE_ROUND_ROBIN = 2, SHUFFLE_RANGE = 3 };   // PhysicalRepartition oneof (auron.proto:629-655)
 
 struct PlanNode {
@@ -150,6 +150,9 @@ struct PlanNode {
   std::vector<SortExprDef> sort_exprs;
   bool sort_has_fetch = false;
   uint64_t sort_fetch = 0;
+  // N_EXPAND (ExpandExecNode, auron.proto:714-722): one expression per schema field in every projection, resolved against
+  // the input schema, of exactly the field's type (expressions beyond the field count are dropped at decode)
+  std::vector<std::vector<ExprP>> expand_projections;
 };
 using PlanP = std::shared_ptr<PlanNode>;
 

@@ -576,6 +576,26 @@ __device__ __forceinline__ void dec_minmax(unsigned long long* key_entry, unsign
   atomicAnd(flags, ~FLAG_SLOT_LOCK);
 }
 
+__device__ __forceinline__ void acc_apply(uint8_t kind, unsigned long long* ke, unsigned long long* w, const uint64_t* arg) {
+  switch (kind) {
+    case ACC_ADD_I64: red_add_u64(w, arg[0]); break;
+    case ACC_ADD_F64: red_add_f64(w, as_f64(arg[0])); break;
+    case ACC_ADD_DEC: {
+      const unsigned long long old = atomicAdd(w, (unsigned long long)arg[0]);
+      const unsigned long long carry = (old + arg[0]) < old ? 1ULL : 0ULL;     // exact: every carry is counted once, adds commute
+      red_add_u64(w + 1, arg[1] + carry);
+      break;
+    }
+    case ACC_COUNT: red_add_u64(w, 1ULL); break;
+    case ACC_MIN_I64: red_min_s64(w, (long long)arg[0]); break;
+    case ACC_MAX_I64: red_max_s64(w, (long long)arg[0]); break;
+    case ACC_MIN_F64: red_min_s64(w, total_order_key(arg[0])); break;
+    case ACC_MAX_F64: red_max_s64(w, total_order_key(arg[0])); break;
+    case ACC_MIN_DEC: dec_minmax(ke, w, mk128(arg[0], arg[1]), true); break;
+    default: dec_minmax(ke, w, mk128(arg[0], arg[1]), false); break;
+  }
+}
+
 // find-or-insert the key, then apply every accumulator update; returns false when the row had to be deferred
 __device__ __forceinline__ bool agg_upsert(const AggLayout& lay, const AggTable& tab, const uint64_t* buf, uint32_t vb) {
   uint64_t kw[AGG_MAX_KEYS * 2];
@@ -596,24 +616,46 @@ __device__ __forceinline__ bool agg_upsert(const AggLayout& lay, const AggTable&
     bool valid = true;
     for (int i = 0; i < a.nargs; i++) valid = valid && ((vb >> a.arg_out[i]) & 1);
     if (!valid) continue;
-    unsigned long long* w = ae + a.word;
-    switch (a.kind) {
-      case ACC_ADD_I64: red_add_u64(w, arg[0]); break;
-      case ACC_ADD_F64: red_add_f64(w, as_f64(arg[0])); break;
-      case ACC_ADD_DEC: {
-        const unsigned long long old = atomicAdd(w, (unsigned long long)arg[0]);
-        const unsigned long long carry = (old + arg[0]) < old ? 1ULL : 0ULL;     // exact: every carry is counted once, adds commute
-        red_add_u64(w + 1, arg[1] + carry);
-        break;
-      }
-      case ACC_COUNT: red_add_u64(w, 1ULL); break;
-      case ACC_MIN_I64: red_min_s64(w, (long long)arg[0]); break;
-      case ACC_MAX_I64: red_max_s64(w, (long long)arg[0]); break;
-      case ACC_MIN_F64: red_min_s64(w, total_order_key(arg[0])); break;
-      case ACC_MAX_F64: red_max_s64(w, total_order_key(arg[0])); break;
-      case ACC_MIN_DEC: dec_minmax(ke, w, mk128(arg[0], arg[1]), true); break;
-      default: dec_minmax(ke, w, mk128(arg[0], arg[1]), false); break;
+    acc_apply(a.kind, ke, ae + a.word, arg);
+    slot_mark(ke, flags, a.vbit);
+  }
+  return true;
+}
+
+// agg_upsert for one grouping set: constant keys come from the set's descriptor, arguments from the set's VM outputs
+__device__ __forceinline__ bool agg_upsert_set(const AggLayout& lay, const AggTable& tab, const uint64_t* buf, uint32_t vb, const AggSetDesc* __restrict__ sd) {
+  uint64_t kw[AGG_MAX_KEYS * 2];
+  uint32_t knull = 0;
+  int w = 0;
+  for (int k = 0; k < lay.nkeys; k++) {
+    const int o = sd->key_out[k];
+    if (o == AGG_KEY_CONST) {
+      const bool null = (sd->key_null >> k) & 1;
+      if (null) knull |= 1u << k;
+      for (int i = 0; i < lay.key_nwords[k]; i++, w++) kw[w] = null ? 0 : sd->key_const[w];
+    } else {
+      const bool valid = (vb >> o) & 1;
+      if (!valid) knull |= 1u << k;
+      for (int i = 0; i < lay.key_nwords[k]; i++) kw[w++] = valid ? buf[lay.out_word[o] + i] : 0;
     }
+  }
+  const uint64_t h = agg_hash_words(kw, w, knull);
+  unsigned flags;
+  bool inserted = false;
+  const uint64_t slot = agg_find_or_insert(lay, tab, kw, knull, h, &flags, &inserted);
+  if (slot == AGG_NO_SLOT) return false;
+  if (inserted) atomicAdd(tab.counters, 1ULL);
+  unsigned long long* const ke = tab.keys + slot * (uint64_t)lay.kstride;
+  unsigned long long* const ae = tab.accs + slot * (uint64_t)lay.astride;
+  const uint32_t skip = sd->acc_skip;
+  for (int j = 0; j < lay.nacc; j++) {
+    if ((skip >> j) & 1) continue;
+    const AccOp a = lay.acc[j];
+    bool valid = true;
+    for (int i = 0; i < 4; i++) { const int o = sd->acc_arg[j][i]; if (o != AGG_NO_ARG) valid = valid && ((vb >> o) & 1); }
+    if (!valid) continue;
+    const int o = sd->acc_arg[j][0];
+    acc_apply(a.kind, ke, ae + a.word, buf + lay.out_word[o == AGG_NO_ARG ? 0 : o]);
     slot_mark(ke, flags, a.vbit);
   }
   return true;
@@ -652,6 +694,48 @@ __global__ void __launch_bounds__(AG_BLOCK) agg_update_kernel(const VmProgram* _
   }
 }
 
+// Expand fused into the aggregate: one VM evaluation per row, then one upsert per grouping set.  A replay list entry is
+// row * nsets + set and replays that set only, so sets of the row that already landed are not counted twice.
+__global__ void __launch_bounds__(AG_BLOCK) agg_update_sets_kernel(const VmProgram* __restrict__ prog, const ColTable cols, const AggLayout lay, const AggTable tab,
+                                                                   long long row_begin, long long n, const uint32_t* __restrict__ row_list,
+                                                                   const AggSetDesc* __restrict__ sets, int nsets) {
+  __shared__ VmInstr s_code[VM_MAX_CODE];
+  __shared__ uint64_t s_pool[VM_MAX_POOL];
+  load_program(prog, s_code, s_pool);
+  int* err = (int*)(tab.counters + 2);
+  const long long ntiles = (n + AG_TILE - 1) / AG_TILE;
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    long long row[AG_R]; bool inb[AG_R], alive[AG_R];
+    uint32_t rel[AG_R]; int only[AG_R];
+#pragma unroll
+    for (int r = 0; r < AG_R; r++) {
+      const long long i = tile * AG_TILE + r * AG_BLOCK + threadIdx.x;
+      inb[r] = i < n; alive[r] = inb[r];
+      const uint32_t e = inb[r] ? (row_list ? row_list[i] : (uint32_t)i) : 0;
+      rel[r] = row_list ? e / (uint32_t)nsets : e;
+      only[r] = row_list ? (int)(e % (uint32_t)nsets) : -1;
+      row[r] = row_begin + rel[r];
+    }
+    uint64_t buf[AG_R][AGG_MAX_ROW_WORDS];
+    uint32_t vb[AG_R];
+#pragma unroll
+    for (int r = 0; r < AG_R; r++) vb[r] = 0;
+    AggSink sink{buf, vb, lay.out_word};
+    vm_run<AG_R>(s_code, s_pool, 0, cols, row, inb, alive, err, sink);
+#pragma unroll
+    for (int r = 0; r < AG_R; r++) {
+      if (!alive[r]) continue;
+      const int s0 = only[r] < 0 ? 0 : only[r], s1 = only[r] < 0 ? nsets : only[r] + 1;
+      for (int s = s0; s < s1; s++) {
+        if (!agg_upsert_set(lay, tab, buf[r], vb[r], sets + s)) {
+          const unsigned long long at = atomicAdd(tab.counters + 1, 1ULL);
+          tab.deferred[at] = rel[r] * (uint32_t)nsets + (uint32_t)s;
+        }
+      }
+    }
+  }
+}
+
 static int grid_for(int64_t ntiles, int per_sm) {
   int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t cap = (int64_t)sms * per_sm;       // grid = multiple of the SM count (persistent, grid-stride)
@@ -663,6 +747,14 @@ int launch_agg_update(const VmProgram* d_prog, const ColTable& cols, const AggLa
   if (n <= 0) return 0;
   const int64_t ntiles = (n + AG_TILE - 1) / AG_TILE;
   agg_update_kernel<<<grid_for(ntiles, 8), AG_BLOCK, 0, s>>>(d_prog, cols, lay, tab, row_begin, n, d_row_list);
+  return 1;
+}
+
+int launch_agg_update_sets(const VmProgram* d_prog, const ColTable& cols, const AggLayout& lay, const AggTable& tab, int64_t row_begin, int64_t n,
+                           const uint32_t* d_row_list, const AggSetDesc* d_sets, int nsets, cudaStream_t s) {
+  if (n <= 0) return 0;
+  const int64_t ntiles = (n + AG_TILE - 1) / AG_TILE;
+  agg_update_sets_kernel<<<grid_for(ntiles, 8), AG_BLOCK, 0, s>>>(d_prog, cols, lay, tab, row_begin, n, d_row_list, d_sets, nsets);
   return 1;
 }
 

@@ -49,13 +49,26 @@ struct AggLayout {
   uint32_t init_flags;               // accumulator-valid bits set at insertion (accumulators with vbit == 0xFF have none)
 };
 
+// Grouping sets of an ExpandExec fused into the aggregate: every row is evaluated once by the VM, then inserted once per set.
+// One descriptor per set lives in device memory next to the program; the key entry layout (AggLayout) is shared by all sets.
+constexpr int AGG_MAX_SETS = 64;
+constexpr uint8_t AGG_KEY_CONST = 0xFF;   // key_out: the key is a constant of the set (key_const words, or NULL in key_null)
+constexpr uint8_t AGG_NO_ARG = 0xFF;
+struct AggSetDesc {
+  uint8_t key_out[AGG_MAX_KEYS];          // VM output of key k in this set, or AGG_KEY_CONST
+  uint8_t acc_arg[AGG_MAX_ACC][4];        // VM output of each argument of accumulator j in this set (AGG_NO_ARG: none)
+  uint32_t key_null;                      // constant keys that are NULL in this set
+  uint32_t acc_skip;                      // accumulators this set never updates (an argument is a NULL literal)
+  uint64_t key_const[AGG_MAX_KEYS * 2];   // words of the constant keys, at their position in the key entry (key_word - 1)
+};
+
 struct AggTable {
   unsigned long long* keys;       // capacity * kstride words
   unsigned long long* accs;       // capacity * astride words
   uint64_t capacity;        // any size: slot = mulhi64(hash, capacity), linear probing with wrap-around
   uint64_t max_groups;      // load limit: inserts beyond it are deferred (table grown by the host, rows replayed)
   unsigned long long* counters;   // [0] ngroups, [1] ndeferred, [2] (int) error flags
-  uint32_t* deferred;       // row indices that could not be inserted
+  uint32_t* deferred;       // row indices that could not be inserted (with grouping sets: row * nsets + set)
 };
 
 // emit descriptors: one per output column
@@ -109,6 +122,9 @@ int64_t filter_project_lean_scratch_bytes(int64_t n);
 
 int launch_agg_update(const VmProgram* d_prog, const ColTable& cols, const AggLayout& lay, const AggTable& tab, int64_t row_begin, int64_t n,
                       const uint32_t* d_row_list /*replay of deferred rows, or null*/, cudaStream_t s);
+// grouping sets: d_row_list entries (and the deferred entries it writes) are row * nsets + set; n counts rows, or list entries
+int launch_agg_update_sets(const VmProgram* d_prog, const ColTable& cols, const AggLayout& lay, const AggTable& tab, int64_t row_begin, int64_t n,
+                           const uint32_t* d_row_list, const AggSetDesc* d_sets, int nsets, cudaStream_t s);
 int launch_agg_rehash(const AggLayout& lay, const AggTable& old_tab, const AggTable& new_tab, cudaStream_t s);
 int launch_agg_emit(const AggLayout& lay, const AggTable& tab, const EmitTable& emit, unsigned long long* d_out_count, cudaStream_t s);
 int launch_pack_valid(const uint8_t* bytes, uint32_t* bits, int64_t n, cudaStream_t s);

@@ -617,6 +617,33 @@ PlanP parse_sort(Reader r) {                 // SortExecNode{input=1, expr=2 (Ph
   return n;
 }
 
+// ExpandExecNode{input=1, schema=2, projections=3}, ExpandProjection{expr=1} (from_proto.rs:518-534) validated like
+// ExpandExec::try_new (expand_exec.rs:49-77)
+PlanP parse_expand(Reader r) {
+  auto n = std::make_shared<PlanNode>(); n->kind = N_EXPAND;
+  bool have_schema = false; std::vector<Reader> projs;
+  while (!r.done()) {
+    int wt; uint32_t f = r.tag(wt);
+    if (f == 1) n->input = parse_plan(r.bytes()); else if (f == 2) { n->schema = parse_schema(r.bytes()); have_schema = true; }
+    else if (f == 3) projs.push_back(r.bytes()); else r.skip(wt);
+  }
+  if (!n->input || !have_schema) bad("Missing required field in protobuf");
+  const SchemaDef& in = n->input->schema;
+  for (auto& pr : projs) {
+    std::vector<ExprP> exprs;
+    Reader pp = pr;
+    while (!pp.done()) { int wt; uint32_t f = pp.tag(wt); if (f == 1) exprs.push_back(parse_expr(pp.bytes(), in)); else pp.skip(wt); }
+    for (size_t i = 0; i < n->schema.fields.size(); i++) {
+      const DType& want = n->schema.fields[i].type;
+      if (i >= exprs.size() || exprs[i]->type != want)
+        bad("ExpandExec data type not matches: " + (i < exprs.size() ? "Some(" + exprs[i]->type.str() + ")" : std::string("None")) + " vs " + want.str());
+    }
+    exprs.resize(n->schema.fields.size());              // execute_expand zips the expressions with the schema fields
+    n->expand_projections.push_back(std::move(exprs));
+  }
+  return n;
+}
+
 // the `~TABLE` column the reference appends to the build side's batches (joins/join_hash_map.rs:409-431, 459-465)
 SchemaDef join_hash_map_schema(const SchemaDef& data) {
   SchemaDef s = data;
@@ -686,7 +713,8 @@ PlanP parse_plan(Reader r) {                  // PhysicalPlanNode oneof (auron.p
       case 15: return parse_leaf(r.bytes(), false);
       case 16: return parse_agg(r.bytes());
       case 18: return parse_leaf(r.bytes(), true);
-      case 1: case 3: case 4: case 9: case 10: case 14: case 17: case 19: case 20:
+      case 20: return parse_expand(r.bytes());
+      case 1: case 3: case 4: case 9: case 10: case 14: case 17: case 19:
       case 21: case 22: case 23: case 24: case 25:
         unsupported("plan node #" + std::to_string(f) + " is outside the Filter/Project/Agg hot path (SURVEY.md §8)");
       default: r.skip(wt);
@@ -766,6 +794,15 @@ static void explain_rec(const PlanP& p, int depth, std::ostringstream& o) {
         o << "):" << a.data_type.str() << "/" << md[a.mode] << " AS " << a.field_name;
       }
       o << "] partial_skipping=" << (p->supports_partial_skipping ? "true" : "false") << " schema=" << schema_str(p->schema) << "\n"; break;
+    }
+    case N_EXPAND: {
+      o << ind << "ExpandExec projections=[";
+      for (size_t j = 0; j < p->expand_projections.size(); j++) {
+        o << (j ? ", " : "") << "[";
+        for (size_t i = 0; i < p->expand_projections[j].size(); i++) o << (i ? ", " : "") << explain_expr(p->expand_projections[j][i]) << " AS " << p->schema.fields[i].name;
+        o << "]";
+      }
+      o << "] schema=" << schema_str(p->schema) << "\n"; break;
     }
     case N_SORT: {
       o << ind << "SortExec [";

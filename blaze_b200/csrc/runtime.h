@@ -98,8 +98,15 @@ class Stage {
 
 std::unique_ptr<Stage> make_filter_project_stage(OpContext& cx, const SchemaDef& in_schema, const std::vector<ExprP>& filters,
                                                  const std::vector<ExprP>& outs, const SchemaDef& out_schema);
+// ExpandExec not fused into an aggregate: every pushed batch yields one batch per projection, in order (expand_exec.rs:147-187)
+std::unique_ptr<Stage> make_expand_stage(OpContext& cx, const SchemaDef& in_schema, const std::vector<ExprP>& filters,
+                                         const std::vector<std::vector<ExprP>>& projections, const SchemaDef& out_schema);
+// one projection of an ExpandExec fused below AggExec(Partial): its grouping keys and aggregate arguments over the stage input
+struct AggSetExprs { std::vector<ExprP> group_exprs; std::vector<std::vector<ExprP>> agg_args; };
+// `sets` (two or more): every input row is inserted once per set; empty: group_exprs / agg_args are the one set
 std::unique_ptr<Stage> make_agg_stage(OpContext& cx, const SchemaDef& in_schema, const std::vector<ExprP>& filters, const PlanNode& agg,
-                                      const std::vector<ExprP>& group_exprs, const std::vector<std::vector<ExprP>>& agg_args);
+                                      const std::vector<ExprP>& group_exprs, const std::vector<std::vector<ExprP>>& agg_args,
+                                      const std::vector<AggSetExprs>& sets = {});
 
 // ShuffleWriterExec (shuffle_stage.cu): terminal stage; its result is the two shuffle files and/or the encoded chunks
 std::unique_ptr<Stage> make_shuffle_write_stage(OpContext& cx, const SchemaDef& in_schema, const PlanNode& node);

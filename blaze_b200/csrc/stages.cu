@@ -269,6 +269,30 @@ std::unique_ptr<Stage> make_filter_project_stage(OpContext& cx, const SchemaDef&
 }
 
 // ---------------------------------------------------------------------------------------------------
+// ExpandStage: one FilterProjectStage per projection, run in order over every pushed batch (the pending filters below the Expand
+// are evaluated by each of them).  Outputs that share the input's buffers hold their own references, so `in` outlives them all.
+// ---------------------------------------------------------------------------------------------------
+class ExpandStage : public Stage {
+  std::vector<std::unique_ptr<FilterProjectStage>> sets_;
+ public:
+  ExpandStage(OpContext& cx, const SchemaDef& in, const std::vector<ExprP>& filters, const std::vector<std::vector<ExprP>>& projections, const SchemaDef& out) {
+    in_schema = in; out_schema = out;
+    for (auto& p : projections) {
+      sets_.emplace_back(new FilterProjectStage(cx, in, filters, p, out));
+      for (int c : sets_.back()->used_input_cols) if (std::find(used_input_cols.begin(), used_input_cols.end(), c) == used_input_cols.end()) used_input_cols.push_back(c);
+    }
+    std::sort(used_input_cols.begin(), used_input_cols.end());
+  }
+  void push(OpContext& cx, DevBatch& in, std::vector<DevBatch>& outs) override { for (auto& s : sets_) s->push(cx, in, outs); }
+  void finish(OpContext&, std::vector<DevBatch>&) override {}
+};
+
+std::unique_ptr<Stage> make_expand_stage(OpContext& cx, const SchemaDef& in_schema, const std::vector<ExprP>& filters,
+                                         const std::vector<std::vector<ExprP>>& projections, const SchemaDef& out_schema) {
+  return std::unique_ptr<Stage>(new ExpandStage(cx, in_schema, filters, projections, out_schema));
+}
+
+// ---------------------------------------------------------------------------------------------------
 // AggStage
 // ---------------------------------------------------------------------------------------------------
 static uint64_t host_mix64(uint64_t x) { x ^= x >> 33; x *= 0xff51afd7ed558ccdULL; x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ULL; x ^= x >> 33; return x; }
@@ -333,6 +357,21 @@ static ExprP strip_noop_casts(ExprP e) {
   return e;
 }
 
+// NULL whatever the row: a NULL literal, through any casts
+static bool is_null_literal(ExprP e) {
+  while (e->kind == E_CAST || e->kind == E_TRY_CAST) e = e->children[0];
+  return e->kind == E_LITERAL && (e->lit_null || e->type.id == T_NULL);
+}
+// a grouping key that is one value for every row of a grouping set (the rolled-up NULLs and the grouping id of an Expand):
+// folded into the set's constant key words, in the representation the VM gives the same value
+static bool const_key(const ExprP& e0, bool& null, uint64_t& lo, uint64_t& hi) {
+  if (is_null_literal(e0)) { null = true; lo = hi = 0; return true; }
+  const ExprP e = strip_noop_casts(e0);
+  if (e->kind != E_LITERAL || !(e->type.is_intlike() || e->type.is_decimal())) return false;
+  null = false; lo = e->lit_lo; hi = e->lit_hi;
+  return true;
+}
+
 // Small pinned host slots (counter snapshots).  cudaMallocHost / cudaFreeHost cost milliseconds once tens of GB are mapped in the process, so
 // ops never call them on their own: one pinned page per process, 32-byte slots, recycled.
 class PinnedSlots {
@@ -362,6 +401,10 @@ class AggStage : public Stage {
   int n_in_ = 0;                        // input columns
   std::vector<FieldDef> merge_state_fields_;   // state columns fed by the merge-mode aggs (in agg order)
   int first_state_col_ = 0;             // index of the first state column in the program's column space
+  // grouping sets of a fused ExpandExec (nsets_ > 1): per-set keys and arguments over the shared VM outputs
+  int nsets_ = 1;
+  std::vector<AggSetDesc> sets_;
+  DevMemP d_sets_;
 
   // table
   DevMemP keys_, accs_, counters_, deferred_[2];
@@ -388,6 +431,8 @@ class AggStage : public Stage {
   int add_out(const ExprP& e) {
     ExprP s = strip_noop_casts(e);
     for (size_t i = 0; i < vm_outs_.size(); i++) if (same_expr(vm_outs_[i], s)) return (int)i;
+    if (nsets_ > 1 && (int)vm_outs_.size() >= VM_MAX_OUT)
+      throw PlanError(B200Q_ERR_UNSUPPORTED, "ExpandExec below AggExec: the grouping sets need more than " + std::to_string(VM_MAX_OUT) + " distinct key and argument expressions (VM_MAX_OUT)");
     vm_outs_.push_back(s);
     return (int)vm_outs_.size() - 1;
   }
@@ -396,7 +441,7 @@ class AggStage : public Stage {
 
  public:
   AggStage(OpContext& cx, const SchemaDef& in, const std::vector<ExprP>& filters, const PlanNode& agg,
-           const std::vector<ExprP>& group_exprs, const std::vector<std::vector<ExprP>>& agg_args) : node_(agg), filters_(filters) {
+           const std::vector<ExprP>& group_exprs, const std::vector<std::vector<ExprP>>& agg_args, const std::vector<AggSetExprs>& sets) : node_(agg), filters_(filters) {
     in_schema = in; out_schema = agg.schema;
     n_in_ = (int)in.fields.size();
     merge_mode_ = agg.need_partial_merge; final_ = agg.need_final_merge;
@@ -406,6 +451,15 @@ class AggStage : public Stage {
     }
     if ((int)group_exprs.size() > AGG_MAX_KEYS) throw PlanError(B200Q_ERR_UNSUPPORTED, "more than 8 grouping columns");
     if (merge_mode_ && !filters.empty()) throw PlanError(B200Q_ERR_UNSUPPORTED, "Filter fused below a merge-mode aggregate");
+    const bool multi = sets.size() > 1;
+    if (multi) {
+      if ((int)sets.size() > AGG_MAX_SETS)
+        throw PlanError(B200Q_ERR_UNSUPPORTED, "ExpandExec below AggExec: " + std::to_string(sets.size()) + " projections exceed the limit of " + std::to_string(AGG_MAX_SETS) + " grouping sets (AGG_MAX_SETS)");
+      if (merge_mode_) throw PlanError(B200Q_ERR_UNSUPPORTED, "ExpandExec fused below a merge-mode aggregate");
+      nsets_ = (int)sets.size();
+      sets_.resize(nsets_);
+      for (auto& d : sets_) { memset(&d, 0, sizeof(d)); memset(d.acc_arg, AGG_NO_ARG, sizeof(d.acc_arg)); }
+    }
 
     // ---- state columns consumed by merge-mode aggs
     for (auto& a : agg.aggs) if (a.mode != MODE_PARTIAL) for (auto& f : state_columns_of(a).fields) merge_state_fields_.push_back(f);
@@ -429,11 +483,25 @@ class AggStage : public Stage {
     int word = 1;
     for (int k = 0; k < lay_.nkeys; k++) {
       const ExprP& g = group_exprs[k];
-      lay_.key_out[k] = (uint8_t)add_out(g);
-      if (lay_.key_out[k] != k) throw PlanError(B200Q_ERR_UNSUPPORTED, "duplicate grouping expressions");
+      if (!multi) {
+        lay_.key_out[k] = (uint8_t)add_out(g);
+        if (lay_.key_out[k] != k) throw PlanError(B200Q_ERR_UNSUPPORTED, "duplicate grouping expressions");
+      } else lay_.key_out[k] = AGG_KEY_CONST;                      // per set: sets_[s].key_out[k]
       lay_.key_word[k] = (uint8_t)word; lay_.key_nwords[k] = g->type.is_decimal() ? 2 : 1;
       word += lay_.key_nwords[k];
     }
+    // grouping sets: a key that is a literal in a set is folded into the set's constant words; every other key expression is a
+    // (deduplicated) VM output, so two key positions of one set may share one output and still keep their own key words
+    for (int s = 0; multi && s < nsets_; s++)
+      for (int k = 0; k < lay_.nkeys; k++) {
+        AggSetDesc& d = sets_[s];
+        bool null = false; uint64_t lo = 0, hi = 0;
+        if (const_key(sets[s].group_exprs[k], null, lo, hi)) {
+          d.key_out[k] = AGG_KEY_CONST;
+          if (null) d.key_null |= 1u << k;
+          else { d.key_const[lay_.key_word[k] - 1] = lo; if (lay_.key_nwords[k] == 2) d.key_const[lay_.key_word[k]] = hi; }
+        } else d.key_out[k] = (uint8_t)add_out(sets[s].group_exprs[k]);
+      }
     lay_.nkw = word - 1;
     const int key_entry_words = word;
     word = 0;                                                     // from here on `word` counts words of the accumulator entry
@@ -473,10 +541,20 @@ class AggStage : public Stage {
         ExprP arg;
         if (partial) { arg = agg_args[ai][0]; }
         else { arg = state_col_expr(state_columns_of(a).fields[0]); }
-        const int o = add_out(arg);
+        // grouping sets: each set's argument is its own VM output; a set whose argument is a NULL literal skips the accumulator
+        std::vector<int> set_o(nsets_, -1);
+        bool set_nullable = false;
+        for (int s = 0; multi && s < nsets_; s++) {
+          const ExprP& e = sets[s].agg_args[ai][0];
+          if (is_null_literal(e)) { set_nullable = true; continue; }
+          set_o[s] = add_out(e); set_nullable = set_nullable || can_be_null(e);
+        }
+        int o = 0;
+        if (!multi) o = add_out(arg);
+        else for (int s = nsets_ - 1; s >= 0; s--) if (set_o[s] >= 0) o = set_o[s];
         // no-grouping aggregates always emit one (pre-seeded) row: with no valid input the accumulator stays NULL
         // (AccPrimColumn valids stay false, agg_exec.rs:280-323), so it needs a validity bit even for never-NULL arguments
-        const bool nullable_arg = can_be_null(arg) || lay_.nkeys == 0;
+        const bool nullable_arg = (multi ? set_nullable : can_be_null(arg)) || lay_.nkeys == 0;
         const uint8_t vbit = nullable_arg ? new_vbit() : (uint8_t)0xFF;
         AccKind kind; int nwords = 1; uint64_t ilo = 0, ihi = 0;
         if (a.fn == AGG_SUM || a.fn == AGG_AVG) {
@@ -492,10 +570,30 @@ class AggStage : public Stage {
           else throw PlanError(B200Q_ERR_UNSUPPORTED, "min/max over " + dt.str() + " is not on the hot path");
         }
         sum_word = add_acc(kind, nwords, vbit, {o}, ilo, ihi); sum_vbit = vbit;
+        for (int s = 0; multi && s < nsets_; s++) {
+          if (set_o[s] < 0) sets_[s].acc_skip |= 1u << (lay_.nacc - 1);
+          else sets_[s].acc_arg[lay_.nacc - 1][0] = (uint8_t)set_o[s];
+        }
       }
       // --- count part (Count, Avg)
       if (a.fn == AGG_COUNT || a.fn == AGG_AVG) {
-        if (partial) {
+        if (multi) {
+          std::vector<std::vector<int>> set_args(nsets_);
+          std::vector<bool> skip(nsets_, false);
+          for (int s = 0; s < nsets_; s++) {
+            const auto& srcs = a.fn == AGG_AVG ? std::vector<ExprP>{sets[s].agg_args[ai][0]} : sets[s].agg_args[ai];
+            for (auto& e : srcs) {
+              if (is_null_literal(e)) skip[s] = true;
+              else if (can_be_null(e)) set_args[s].push_back(add_out(e));
+            }
+            if (set_args[s].size() > 4) throw PlanError(B200Q_ERR_UNSUPPORTED, "count over more than 4 nullable arguments");
+          }
+          cnt_word = add_acc(ACC_COUNT, 1, 0xFF, set_args[0], 0, 0);
+          for (int s = 0; s < nsets_; s++) {
+            if (skip[s]) { sets_[s].acc_skip |= 1u << (lay_.nacc - 1); continue; }
+            for (size_t i = 0; i < set_args[s].size(); i++) sets_[s].acc_arg[lay_.nacc - 1][i] = (uint8_t)set_args[s][i];
+          }
+        } else if (partial) {
           std::vector<int> args;
           const auto& srcs = a.fn == AGG_AVG ? std::vector<ExprP>{agg_args[ai][0]} : agg_args[ai];
           for (auto& e : srcs) if (can_be_null(e)) args.push_back(add_out(e));      // agg.rs:178-189 + never-NULL arguments dropped
@@ -547,14 +645,22 @@ class AggStage : public Stage {
     lay_.nouts = (int)cp_.outs.size();
     int ow = 0;
     for (size_t i = 0; i < cp_.outs.size(); i++) { lay_.out_word[i] = (uint8_t)ow; ow += cp_.outs[i].slots; }
-    if (ow > AGG_MAX_ROW_WORDS) throw PlanError(B200Q_ERR_UNSUPPORTED, "too many key/argument words per row");
+    if (ow > AGG_MAX_ROW_WORDS) {
+      if (multi) throw PlanError(B200Q_ERR_UNSUPPORTED, "ExpandExec below AggExec: the grouping sets need " + std::to_string(ow) + " key/argument words per row, more than " + std::to_string(AGG_MAX_ROW_WORDS) + " (AGG_MAX_ROW_WORDS)");
+      throw PlanError(B200Q_ERR_UNSUPPORTED, "too many key/argument words per row");
+    }
     for (int c : cp_.used_cols) if (c < n_in_) used_input_cols.push_back(c);
     if (merge_mode_ && !columnar_) used_input_cols.push_back(n_in_ - 1);
     std::sort(used_input_cols.begin(), used_input_cols.end());
     used_input_cols.erase(std::unique(used_input_cols.begin(), used_input_cols.end()), used_input_cols.end());
     d_prog_ = upload_program(cp_, cx.stream);
+    if (multi) {                              // the set descriptors travel next to the program (they do not fit the kernel parameters)
+      d_sets_ = DevMem::alloc(sizeof(AggSetDesc) * sets_.size(), cx.stream);
+      B200Q_CUDA(cudaMemcpyAsync(d_sets_->ptr, sets_.data(), sizeof(AggSetDesc) * sets_.size(), cudaMemcpyHostToDevice, cx.stream));
+    }
 
-    if (!cp_.has_strings) {                   // the specialised kernels read fixed-width columns only: string programs stay on the VM kernel
+    if (!cp_.has_strings && !multi) {         // the specialised kernels read fixed-width columns only: string programs stay on the VM kernel;
+                                              // they insert one key per row, so grouping sets stay on the VM kernel too
       detect_fast(cx);
       if (!fast_ok_) detect_wide(cx);
     }
@@ -949,6 +1055,7 @@ class AggStage : public Stage {
   }
 
   int launch_update(OpContext& cx, const ColTable& ct, const AggTable& t, int64_t begin, int64_t m, const uint32_t* list) {
+    if (nsets_ > 1) return launch_agg_update_sets((const VmProgram*)d_prog_->ptr, ct, lay_, t, begin, m, list, (const AggSetDesc*)d_sets_->ptr, nsets_, cx.stream);
     // deferred-row replays (arbitrary row lists, rare) always take the generic kernel: same table, same semantics
     if (wide_possible_ && ws_.dense_tab && !list) {
       cx.m.fast_launches++;
@@ -1073,15 +1180,18 @@ class AggStage : public Stage {
   }
 
   void update_rows(OpContext& cx, const ColTable& ct, int64_t n) {
-    const int64_t chunk = std::max<int64_t>(1 << 16, std::min<int64_t>(cx.conf.max_launch_rows, 0x7FFFFFFFLL));
+    int64_t chunk = std::max<int64_t>(1 << 16, std::min<int64_t>(cx.conf.max_launch_rows, 0x7FFFFFFFLL));
+    // grouping sets: a launch inserts rows x sets keys; its rows are clamped so that a deferred entry (row * nsets + set) fits in 32 bits
+    // and the deferred buffers stay as large as a single-set launch of `chunk` rows would make them
+    if (nsets_ > 1) chunk = std::max<int64_t>(1 << 16, chunk / nsets_);
     static const bool dbg = getenv("B200Q_AGG_TIMING") != nullptr;
     auto hnow = [] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
     const double tA = hnow();
     ensure_snaps();
     const double tB = hnow();
     const int64_t m_max = std::min(chunk, n);
-    if (deferred_cap_ < 2 * m_max) {                                      // two chunks' worth: a chunk is launched before the counters of the one before it are back
-      deferred_cap_ = 2 * m_max;
+    if (deferred_cap_ < 2 * m_max * nsets_) {                             // two chunks' worth: a chunk is launched before the counters of the one before it are back
+      deferred_cap_ = 2 * m_max * nsets_;
       deferred_[0] = DevMem::alloc((size_t)deferred_cap_ * 4, cx.stream);
       deferred_[1] = nullptr;
     }
@@ -1242,8 +1352,9 @@ class AggStage : public Stage {
 };
 
 std::unique_ptr<Stage> make_agg_stage(OpContext& cx, const SchemaDef& in_schema, const std::vector<ExprP>& filters, const PlanNode& agg,
-                                      const std::vector<ExprP>& group_exprs, const std::vector<std::vector<ExprP>>& agg_args) {
-  return std::unique_ptr<Stage>(new AggStage(cx, in_schema, filters, agg, group_exprs, agg_args));
+                                      const std::vector<ExprP>& group_exprs, const std::vector<std::vector<ExprP>>& agg_args,
+                                      const std::vector<AggSetExprs>& sets) {
+  return std::unique_ptr<Stage>(new AggStage(cx, in_schema, filters, agg, group_exprs, agg_args, sets));
 }
 
 }  // namespace b200q

@@ -144,6 +144,30 @@ class ProjectExec(ExecutionPlan):
                                  [e.data_type(ins) for e, _ in self.exprs])
 
 
+class ExpandExec(ExecutionPlan):
+    """ExpandExec::try_new(schema, projections, input) (expand_exec.rs:49-77): every input batch yields one output batch per
+    projection, in order.  Each projection needs an expression of the field's exact type for every schema field; expressions
+    beyond the field count are ignored.  Spark plans it below the partial aggregate of ROLLUP / CUBE / GROUPING SETS and of
+    aggregates over several DISTINCT column sets."""
+
+    def __init__(self, schema: Schema, projections: Sequence[Sequence[E.Expr]], input: ExecutionPlan):
+        self._schema = schema
+        self.projections = [list(p) for p in projections]
+        self.input = input
+        self._validate()                                                # the native decoder applies try_new's type checks
+
+    try_new = classmethod(lambda cls, schema, projections, input: cls(schema, projections, input))
+
+    def schema(self):
+        return self._schema
+
+    def children(self):
+        return [self.input]
+
+    def node(self):
+        return P.expand_node(self.input.node(), self._schema, self.projections)
+
+
 def create_agg(function: int, children: Sequence[E.Expr], input_schema: Schema, return_type: T.DataType) -> AggFunctionExpr:
     """`create_agg` (agg/agg.rs:171-205).  The Count/Sum/Avg rewrites (drop non-nullable count
     children, wrap Sum/Avg children in TryCast(return_type)) happen natively at decode time, exactly

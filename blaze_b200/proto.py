@@ -22,8 +22,8 @@ _F = dpb.FieldDescriptorProto
 _PKG = "plan.protobuf"
 
 
-def _msg(fd, name, fields, oneofs=()):
-    m = fd.message_type.add()
+def _msg(fd, name, fields, oneofs=(), into=None):
+    m = (into if into is not None else fd.message_type).add()
     m.name = name
     for o in oneofs:
         m.oneof_decl.add().name = o
@@ -177,8 +177,15 @@ def _build_pool():
         ("hash_join", 11, "HashJoinExecNode", O), ("broadcast_join_build_hash_map", 12, "BroadcastJoinBuildHashMapExecNode", O),
         ("broadcast_join", 13, "BroadcastJoinExecNode", O), ("filter", 8, "FilterExecNode", O),
         ("empty_partitions", 15, "EmptyPartitionsExecNode", O), ("agg", 16, "AggExecNode", O),
-        ("ffi_reader", 18, "FFIReaderExecNode", O),
+        ("ffi_reader", 18, "FFIReaderExecNode", O), ("expand", 20, "PhysicalPlanNode.ExpandExecNode", O),
     ], oneofs=["PhysicalPlanType"])
+    # ExpandExecNode{input=1, schema=2, projections=3} and ExpandProjection{expr=1} (auron.proto:714-722) are top-level in the reference;
+    # nested here like the string-match nodes above (same bytes on the wire), the top-level set stays that of the field table of
+    # tests/golden/auron_proto_fields.json.  tests/test_proto_expand_compat.py checks them against tests/golden/auron_proto_expand_fields.json
+    pp = next(m for m in fd.message_type if m.name == "PhysicalPlanNode")
+    _msg(fd, "ExpandExecNode", [("input", 1, "PhysicalPlanNode"), ("schema", 2, "Schema"), ("projections", 3, "PhysicalPlanNode.ExpandProjection", R)],
+         into=pp.nested_type)
+    _msg(fd, "ExpandProjection", [("expr", 1, "PhysicalExprNode", R)], into=pp.nested_type)
     _msg(fd, "PartitionId", [("stage_id", 2, _F.TYPE_UINT32), ("partition_id", 4, _F.TYPE_UINT32), ("task_id", 5, _F.TYPE_UINT64)])
     _msg(fd, "TaskDefinition", [("task_id", 1, "PartitionId"), ("plan", 2, "PhysicalPlanNode")])
 
@@ -362,6 +369,17 @@ def projection_node(input_node, exprs, names, data_types):
         n.projection.expr.add().CopyFrom(expr_msg(e))
         n.projection.expr_name.append(name)
         n.projection.data_type.add().CopyFrom(arrow_type_msg(dt))
+    return n
+
+
+def expand_node(input_node, schema: Schema, projections):
+    n = PhysicalPlanNode()
+    n.expand.input.CopyFrom(input_node)
+    n.expand.schema.CopyFrom(schema_msg(schema))
+    for proj in projections:
+        p = n.expand.projections.add()
+        for e in proj:
+            p.expr.add().CopyFrom(expr_msg(e))
     return n
 
 

@@ -404,3 +404,54 @@ if any(t in (ONLY or "B1,B2") for t in ("B1", "B2")):
         run_shuffle_wall("B2 q1 map side: Filter -> AggExec(Partial) -> ShuffleWriterExec 200-way, " + ("columnar partial state" if columnar else "reference format (Binary state)"),
                          w, q_spec, [bf, bk1, bk2, bv], native.default_conf(shuffle_output_on_device=1, partial_state_columnar=int(columnar), agg_initial_groups=1 << 20), brows)
     del bf, bk1, bk2, bv
+
+
+# E1-E2: Filter[f < 800] -> Expand ROLLUP(k1, k2) (3 sets) -> AggExec(Partial) SUM(v), COUNT(v) -> AggExec(Final) over four device-resident
+# int64 columns, k1, k2 ~ U[0, 1000).  E1 fuses the Expand into the aggregate (each row read once, one upsert per set); E2 puts a Filter that
+# keeps every row between the Expand and the AggExec, which materialises the 3 projections through the standalone ExpandStage.
+# Timed like B1-B2: push_device -> finish -> sync.  Algorithmic bytes: 32 B/row, the input read once.
+def run_expand_wall(name, plan, spec, keep, conf, n, nsets):
+    if ONLY and not any(t in name for t in ONLY.split(",")): return
+    import time
+    best = None
+    for _ in range(REPS or 3):
+        with native.NativeOp(plan.plan_bytes(), conf, 0) as op:
+            torch.cuda.synchronize(); t0 = time.perf_counter()
+            op.push_device(native.DeviceBatch(spec, n, 0, keepalive=keep))
+            op.finish(); op.sync()
+            dt = time.perf_counter() - t0
+            m = op.metrics(); n_out = 0
+            while True:
+                o = op.pull_device()
+                if o is None: break
+                n_out += o.array.length; native.release_device_array(o)
+        if best is None or dt < best[0]: best = (dt, m, n_out)
+    dt, m, n_out = best
+    print(json.dumps({"shape": name, "rows": n, "sets": nsets, "out_rows": n_out, "wall_ms_push_to_sync": dt * 1e3, "rows_per_s": n / dt,
+                      "row_sets_per_s": n * nsets / dt, "alg_GBps": 32.0 * n / dt / 1e9, "frac_of_hbm_peak": 32.0 * n / dt / 1e9 / peak,
+                      "launches": m["gpu_kernel_launches"], "num_groups": m["num_groups"]}), flush=True)
+
+
+erows = int(os.environ.get("ROWS", 1 << 26))
+if any(t in (ONLY or "E1,E2") for t in ("E1", "E2")):
+    ef = torch.randint(0, 1000, (erows,), dtype=torch.int64, device=dev, generator=g)
+    ek1 = torch.randint(0, 1000, (erows,), dtype=torch.int64, device=dev, generator=g)
+    ek2 = torch.randint(0, 1000, (erows,), dtype=torch.int64, device=dev, generator=g)
+    ev = torch.randint(-10**6, 10**6, (erows,), dtype=torch.int64, device=dev, generator=g)
+    e_sch = T.Schema([T.Field(nm, T.int64, False) for nm in ("k1", "k2", "v", "f")])
+    x_sch = T.Schema([T.Field("k1", T.int64, True), T.Field("k2", T.int64, True), T.Field("v", T.int64, False), T.Field("spark_grouping_id", T.int64, False)])
+    null64 = E.Literal(None, T.int64)
+    e_projs = [[E.Column("k1"), E.Column("k2"), E.Column("v"), E.Literal(0, T.int64)], [E.Column("k1"), null64, E.Column("v"), E.Literal(1, T.int64)],
+               [null64, null64, E.Column("v"), E.Literal(3, T.int64)]]
+    e_g = [E.GroupingExpr(nm, E.Column(nm)) for nm in ("k1", "k2", "spark_grouping_id")]
+    e_aggs = lambda mode, ch: [E.AggExpr("s", mode, PL.create_agg(E.AGG_SUM, ch, x_sch, T.int64)), E.AggExpr("c", mode, PL.create_agg(E.AGG_COUNT, ch, x_sch, T.int64))]
+    e_spec = [(t.data_ptr(), 0, erows) for t in (ek1, ek2, ev, ef)]
+    for fused in (True, False):
+        ex = PL.ExpandExec(x_sch, e_projs, PL.FilterExec([E.BinaryExpr(E.Column("f"), "Lt", E.Literal(800, T.int64))], PL.MemoryExec(e_sch)))
+        below = ex if fused else PL.FilterExec([E.BinaryExpr(E.Column("v"), "GtEq", E.Literal(-10**6, T.int64))], ex)
+        part = PL.AggExec(PL.HashAgg, e_g, e_aggs(E.PARTIAL, [E.Column("v")]), True, below)
+        fin = PL.AggExec(PL.HashAgg, e_g, e_aggs(E.FINAL, [E.placeholder(T.int64)]), False, part)
+        run_expand_wall("E1 Filter -> Expand ROLLUP(k1, k2) fused into AggExec(Partial) -> AggExec(Final)" if fused else
+                        "E2 Filter -> Expand ROLLUP(k1, k2) -> Filter(all rows) -> AggExec(Partial) -> AggExec(Final), standalone Expand",
+                        fin, e_spec, [ef, ek1, ek2, ev], native.default_conf(agg_initial_groups=1 << 20), erows, 3)
+    del ef, ek1, ek2, ev

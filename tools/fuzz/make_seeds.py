@@ -34,7 +34,13 @@ def seed_plans():
     sa = PL.AggExec(PL.HashAgg, [E.GroupingExpr("k", E.Column("k"))],
                     [E.AggExpr("c", E.PARTIAL, PL.create_agg(E.AGG_COUNT, [S_], su, T.int64)),
                      E.AggExpr("n", E.PARTIAL, PL.create_agg(E.AGG_SUM, [E.TryCast(T_, T.int64)], su, T.int64))], False, fs)
-    return [proj.plan_bytes(), partial.plan_bytes(), final.plan_bytes(), ps.plan_bytes(), sa.plan_bytes()]
+    # ExpandExec: ROLLUP(a, b) below AggExec(Partial) (rolled-up keys as typed NULLs, the grouping id as a literal)
+    xs = T.Schema([T.Field("a", T.int64, True), T.Field("b", T.int32, True), T.Field("d", T.decimal128(17, 2), True), T.Field("gid", T.int64, False)])
+    n64, n32 = E.Literal(None, T.int64), E.Literal(None, T.int32)
+    ex = PL.ExpandExec(xs, [[A, B, D, E.Literal(0, T.int64)], [A, n32, D, E.Literal(1, T.int64)], [n64, n32, D, E.Literal(3, T.int64)]], f)
+    xa = PL.AggExec(PL.HashAgg, [E.GroupingExpr(n, E.Column(n)) for n in ("a", "b", "gid")],
+                    [E.AggExpr("s", E.PARTIAL, PL.create_agg(E.AGG_SUM, [E.Column("d")], xs, T.decimal128(27, 2)))], False, ex)
+    return [proj.plan_bytes(), partial.plan_bytes(), final.plan_bytes(), ps.plan_bytes(), sa.plan_bytes(), xa.plan_bytes()]
 
 
 if __name__ == "__main__":
