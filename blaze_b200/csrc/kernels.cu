@@ -18,7 +18,6 @@
 
 #include "agg_device.cuh"
 #include "kernels.cuh"
-#include "tma.cuh"
 #include "vm.cuh"
 #include "emit_device.cuh"
 
@@ -355,117 +354,6 @@ __global__ void __launch_bounds__(FL_BLOCK, OCC) filter_project_lean_kernel(cons
   }
 }
 
-
-// ---- single-pass form with TMA-staged tiles (round 2) ----
-// The two-pass form reads the filter columns twice (M0: 32 B of traffic for 24 algorithmic bytes per row); the ticketed single
-// pass above parks a tile's rows in registers while it waits for its exclusive prefix, with no loads in flight.  Here a tile
-// (2048 rows of every column) is brought into shared memory by cp.async.bulk, the copy of the CTA's NEXT tile is issued before
-// the current one is even counted, and the look-back wait happens with that copy in flight and nothing but eight ballots held
-// in registers; the projected survivors are then read from shared memory and stored in order.  Tiles are assigned round-robin
-// to a grid that is fully resident (the launcher sizes it from the occupancy), so a waiting CTA's predecessors are running.
-#ifndef B200Q_EMULATED_DEVICE
-template <int NC>
-__global__ void __launch_bounds__(FL_BLOCK) filter_project_tma_kernel(const LeanFpDev sp, long long n, long long ntiles, unsigned long long* tile_status, unsigned long long* scratch) {
-  extern __shared__ __align__(16) unsigned char fsm[];
-  long long* stage = (long long*)fsm;                                      // [2][NC][FL_TILE]
-  __shared__ unsigned long long s_bar[2];
-  __shared__ long long s_base[FL_NW];
-  __shared__ unsigned s_cnt[FL_NW];
-  const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  auto issue = [&](long long tile, int buf) {                              // full tiles only: the last, partial tile is read with plain loads
-    if (tile >= ntiles || (tile + 1) * FL_TILE > n) return;
-    mbar_expect_tx(&s_bar[buf], NC * FL_TILE * 8);
-#pragma unroll
-    for (int c = 0; c < NC; c++) bulk_g2s(stage + ((size_t)buf * NC + c) * FL_TILE, sp.col[c] + tile * FL_TILE, FL_TILE * 8, &s_bar[buf]);
-  };
-  if (threadIdx.x == 0) { mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_fence_init(); }
-  __syncthreads();
-  if (threadIdx.x == 0) issue(blockIdx.x, 0);
-  unsigned it = 0;
-  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, it++) {
-    const int buf = it & 1;
-    const bool staged = (tile + 1) * FL_TILE <= n;
-    if (threadIdx.x == 0) issue(tile + gridDim.x, buf ^ 1);                // the other buffer was released by the barrier that ended the previous iteration
-    const long long* st = stage + (size_t)buf * NC * FL_TILE + warp * FL_CHUNK + lane;
-    const long long row0 = tile * FL_TILE + warp * FL_CHUNK + lane;
-    if (staged) mbar_wait(&s_bar[buf], (it >> 1) & 1);
-    // survivors: a ballot per warp-row (the conjuncts' columns come from shared memory, or from HBM for the partial tile)
-    unsigned am[FL_R];
-    unsigned wt = 0;
-    {
-      bool alive[FL_R];
-#pragma unroll
-      for (int r = 0; r < FL_R; r++) alive[r] = row0 + r * 32 < n;
-      for (int f = 0; f < sp.nfilt; f++) {
-        const unsigned mask = sp.filt[f].mask; const long long lit = sp.filt[f].lit; const int slot = sp.filt[f].slot;
-#pragma unroll
-        for (int r = 0; r < FL_R; r++) {
-          const long long x = staged ? st[(size_t)slot * FL_TILE + r * 32] : (alive[r] ? sp.col[slot][row0 + r * 32] : 0);
-          alive[r] = alive[r] && fl_cmp(mask, x, lit);
-        }
-      }
-#pragma unroll
-      for (int r = 0; r < FL_R; r++) { am[r] = __ballot_sync(0xffffffffu, alive[r]); wt += __popc(am[r]); }
-    }
-    if (lane == 0) s_cnt[warp] = wt;
-    __syncthreads();
-    if (warp == 0) {
-      const unsigned v = lane < FL_NW ? s_cnt[lane] : 0;
-      unsigned incl = v;
-#pragma unroll
-      for (int d = 1; d < FL_NW; d <<= 1) { unsigned t = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += t; }
-      const unsigned long long total = __shfl_sync(0xffffffffu, incl, FL_NW - 1);
-      unsigned long long excl = 0;
-      if (tile > 0) {
-        if (lane == 0) st_relaxed_u64(tile_status + tile, ST_AGG | total);
-        long long j = tile - 1;
-        while (true) {                                                     // decoupled look-back, 32 predecessors per round
-          const long long idx = j - lane;
-          unsigned long long stw = idx >= 0 ? ld_relaxed_u64(tile_status + idx) : ST_PREFIX;
-          if (__any_sync(0xffffffffu, (stw >> 62) == 0)) { __nanosleep(32); continue; }
-          const unsigned pm = __ballot_sync(0xffffffffu, (stw >> 62) == 2);
-          unsigned long long val = stw & ST_VALUE;
-          if (pm) { const int first = __ffs(pm) - 1; if ((int)lane > first) val = 0; }
-#pragma unroll
-          for (int d = 16; d > 0; d >>= 1) val += __shfl_xor_sync(0xffffffffu, val, d);
-          excl += val;
-          if (pm) break;
-          j -= 32;
-        }
-      }
-      if (lane == 0) {
-        st_relaxed_u64(tile_status + tile, ST_PREFIX | (excl + total));
-        if (tile == ntiles - 1) scratch[1] = excl + total;
-      }
-      if (lane < FL_NW) s_base[lane] = (long long)(excl + (incl - v));
-    }
-    __syncthreads();
-    // projected survivors, in order, from the staged tile
-    {
-      const unsigned lt = lanemask_lt();
-      const long long wbase = s_base[warp];
-      for (int o = 0; o < sp.nout; o++) {
-        const int kind = sp.out[o].kind, sa = sp.out[o].a, sb = sp.out[o].b;
-        long long* const dst = sp.out[o].dst + wbase;
-        unsigned rank = 0;
-#pragma unroll
-        for (int r = 0; r < FL_R; r++) {
-          if ((am[r] >> lane) & 1) {
-            const long long va = staged ? st[(size_t)sa * FL_TILE + r * 32] : sp.col[sa][row0 + r * 32];
-            const long long vb = sb == 0xFF ? sp.out[o].lit : (staged ? st[(size_t)sb * FL_TILE + r * 32] : sp.col[sb][row0 + r * 32]);
-            const unsigned long long a = (unsigned long long)va, b = (unsigned long long)vb;
-            const unsigned long long v = kind == 0 ? a : kind == 1 ? a + b : kind == 2 ? a - b : a * b;     // wrapping, like the reference
-            dst[rank + __popc(am[r] & lt)] = (long long)v;
-          }
-          rank += __popc(am[r]);
-        }
-      }
-    }
-    __syncthreads();                                                       // every lane is done with this buffer: it may be overwritten
-  }
-}
-#endif
-
 int launch_filter_project_lean(const ColTable& cols, int ncols, const LeanFpSpec& sp, long long* const* out_values, int64_t n,
                                void* d_work /* filter_project_lean_scratch_bytes(n), zeroed */, unsigned long long* d_scratch, cudaStream_t s) {
   if (n <= 0) return 0;
@@ -482,27 +370,6 @@ int launch_filter_project_lean(const ColTable& cols, int ncols, const LeanFpSpec
     d.out[o].kind = sp.out[o].kind; d.out[o].a = (uint8_t)sp.out[o].a; d.out[o].b = sp.out[o].b < 0 ? 0xFF : (uint8_t)sp.out[o].b;
     d.out[o].lit = sp.out[o].lit; d.out[o].dst = out_values[o];
   }
-#ifndef B200Q_EMULATED_DEVICE
-  {   // large batches: the TMA-staged single pass exists (B200Q_FILTER_TMA=1) but is NOT the default: with a fully resident grid walking the
-      // tiles in lockstep, every tile's look-back has to sum the aggregates of a whole wave (hundreds of tiles, a chain of dependent L2
-      // round trips) while a tile is only microseconds of HBM time; the two-pass form streams both passes at HBM speed
-    static const bool two_pass = getenv("B200Q_FILTER_TMA") == nullptr;
-    bool aligned = true;
-    for (int c = 0; c < ncols; c++) aligned = aligned && (((uintptr_t)d.col[c]) & 15) == 0;
-    if (!two_pass && aligned && sp.nfilt && n >= FL_TWO_PASS_MIN_ROWS) {
-      const int64_t ntiles = (n + FL_TILE - 1) / FL_TILE;
-      const size_t smem = (size_t)2 * ncols * FL_TILE * 8;
-      int occ = 0, dev = 0, sms = 132;
-      cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-#define B200Q_FTMA(NC_) do { cudaFuncSetAttribute(filter_project_tma_kernel<NC_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, filter_project_tma_kernel<NC_>, FL_BLOCK, smem); \
-        if (occ > 0) filter_project_tma_kernel<NC_><<<(unsigned)std::min<int64_t>(ntiles, (int64_t)occ * sms), FL_BLOCK, smem, s>>>(d, n, ntiles, (unsigned long long*)d_work, d_scratch); } while (0)
-      switch (ncols) { case 1: B200Q_FTMA(1); break; case 2: B200Q_FTMA(2); break; case 3: B200Q_FTMA(3); break; default: B200Q_FTMA(4); break; }
-#undef B200Q_FTMA
-      if (occ > 0) return 1;
-    }
-  }
-#endif
   if (sp.nfilt && n >= FL_TWO_PASS_MIN_ROWS) {
     const int64_t nch = fl_num_chunks(n);
     int32_t* counts = (int32_t*)d_work; int32_t* offsets = counts + nch; int32_t* sums = offsets + nch + 1;

@@ -1,22 +1,26 @@
 // Descriptors of the specialised HashAgg update kernels (kernels_fast.cu).
 #pragma once
+#include <cstddef>
+
 #include "kernels.cuh"
 
 namespace b200q {
 
 enum FastAccKind : uint8_t { FAST_ACC_ADD = 0, FAST_ACC_COUNT = 1 };   // COUNT with col < 0 is COUNT(*)
 
+// the `col cmp literal` conjuncts on one column merged into one closed interval: a row passes iff (u64)(x - lo) <= span
+struct FilterInterval { int8_t col; uint8_t phys; uint8_t _pad[6]; long long lo; unsigned long long span; };
+
 struct FastSpec {
   int32_t nkeys, nacc, nfilt, dense;
-  int32_t row_kernels;                                    // debugging / A-B measurements: keep the round-1 one-row-per-lane kernels (B200Q_ROW_KERNELS=1)
   int32_t lean, hot_cache;                                // lean: all referenced columns are aligned non-null int64 (set per launch); hot_cache: skewed keys (experimental)
   int8_t key_col[2]; uint8_t key_phys[2];                 // program column slots / physical kinds of the key columns
   struct { uint8_t kind; int8_t col; uint8_t phys; uint8_t vbit; uint8_t word; uint8_t _pad[3]; } acc[2];
   struct { int8_t col; uint8_t phys; uint8_t op; uint8_t _pad[5]; long long lit; } filt[4];
-  // the same conjuncts merged per column into closed intervals (tile kernels): row passes iff (u64)(x - lo) <= span for every column
-  int32_t nfcol;                                          // -1: the conjuncts cannot be merged (a `!=` term or more than 2 columns): tile kernels not used
+  // the same conjuncts merged per column (tile kernels): a row passes iff it lies in every interval
+  int32_t nfcol;                                          // -1: the conjuncts cannot be merged (a `!=` term or more than 2 columns): a dense table takes the row kernels
   int32_t filt_never;                                     // the merged intervals are empty: no row passes
-  struct { int8_t col; uint8_t phys; uint8_t _pad[6]; long long lo; unsigned long long span; } frange[2];
+  FilterInterval frange[2];
   long long dense_base;                                   // DENSE: entry index = key0 - dense_base                      (one key)
   unsigned long long dense_cap;                           // entries of dense_stride words
   long long dense_base1;                                  //        entry index = (key0 - dense_base) * dense_r1 + (key1 - dense_base1)   (two keys)
@@ -71,7 +75,7 @@ struct TileAggSpec {
   int32_t nkeys, nargs, nfcol, filt_never, nacc, G, flavour, arg_is_dec;
   int8_t key_col[2]; uint8_t key_phys[2];
   int8_t arg_col[2]; uint8_t arg_phys[2]; uint8_t arg_cvt[2]; uint8_t arg_values[2];      // arg_values: 0 = only the validity is needed (COUNT(col))
-  struct { int8_t col; uint8_t phys; uint8_t _pad[6]; long long lo; unsigned long long span; } frange[2];
+  FilterInterval frange[2];
   long long dense_base, dense_base1;
   unsigned long long dense_cap, dense_r1, dense_cap0;
   unsigned long long* dense_tab;
@@ -81,6 +85,10 @@ struct TileAggSpec {
   uint8_t presence_word, dec_word /* first of the three decimal pieces, 0xFF: none */, _pad2[6];
   struct { int8_t arg; uint8_t recon; uint8_t w0; uint8_t valid_word; uint8_t lay_acc; uint8_t _pad[3]; } acc[4];
 };
+// the kernels take both descriptors by value as launch parameters: a change of size or interval offset must be deliberate
+static_assert(sizeof(FastSpec) == 232 && offsetof(FastSpec, frange) == 120, "FastSpec layout");
+static_assert(sizeof(TileAggSpec) == 456 && offsetof(TileAggSpec, frange) == 48, "TileAggSpec layout");
+
 int launch_agg_tile_wide(const ColTable& cols, const TileAggSpec& ts, const AggLayout& lay, const AggTable& tab, int64_t row_begin, int64_t n, cudaStream_t s);
 int launch_tile_wide_init(const TileAggSpec& ts, cudaStream_t s);                       // identities of the dense entries
 int launch_tile_wide_count(const TileAggSpec& ts, unsigned long long* d_out, cudaStream_t s);

@@ -665,11 +665,10 @@ int launch_shuffle_encode(const ShufSpec& sp, const uint16_t* d_pids, int64_t n,
 #ifndef B200Q_EMULATED_DEVICE
   // the bulk-copy staging costs 64 KB more shared memory per CTA (a smaller L1 for the write-combining of the byte stores) but takes
   // the column loads off the warps' critical path; on H100 it is the faster form (bench.py M3, 200-way, 2^28 rows: 26.7 ms against
-  // 30.4-31.2 ms per step, H100 SXM 80 GB at 700 W), so it is the default; B200Q_SHUFFLE_TMA=0 selects the register-staged form
-  static const bool no_tma = [] { const char* e = getenv("B200Q_SHUFFLE_TMA"); return e != nullptr && e[0] == '0'; }();
+  // 30.4-31.2 ms per step, H100 SXM 80 GB at 700 W), so every column it can take uses it
   for (int c = 0; c < spx.ncols; c++) {                                                     // bulk copies need 16-byte aligned sources
     ShufCol& col = spx.col[c];
-    col.tma = !no_tma && (col.width == 1 || col.width == 2 || col.width == 4 || col.width == 8) && ((uintptr_t)col.values & 15) == 0 && n >= SHUF_TILE;
+    col.tma = (col.width == 1 || col.width == 2 || col.width == 4 || col.width == 8) && ((uintptr_t)col.values & 15) == 0 && n >= SHUF_TILE;
     tma = tma || col.tma;
   }
 #endif

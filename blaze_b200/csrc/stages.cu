@@ -678,7 +678,7 @@ class AggStage : public Stage {
     // capacity: any size (slot = mulhi(hash, capacity)); sized for a load of ~0.6 at the hinted group count so that
     // key area + accumulator area stay L2-resident; floor 2^20 keeps the slack above the load limit (0.3 * capacity)
     // larger than the concurrent-insert overshoot bound (resident threads ~ 303K)
-    capacity_ = std::max<uint64_t>(1ULL << 20, (uint64_t)((double)std::max<int64_t>(cx.conf.agg_initial_groups, 1) * cap_factor()));
+    capacity_ = std::max<uint64_t>(1ULL << 20, (uint64_t)((double)std::max<int64_t>(cx.conf.agg_initial_groups, 1) * AGG_SLOTS_PER_GROUP));
     if (capacity_ >= (1ULL << 32)) throw PlanError(B200Q_ERR_UNSUPPORTED, "agg_initial_groups too large");
     alloc_table(cx, capacity_, keys_, accs_, counters_);
     if (lay_.nkeys == 0) seed_global_group(cx);
@@ -694,18 +694,38 @@ class AggStage : public Stage {
   }
   static bool int_phys(const DType& t) { return t.is_intlike(); }
 
+  // the 1-2 integer key columns and the `col cmp literal` conjuncts of the specialised kernels (key slots, filt[], merged
+  // into frange[] by merge_conjuncts); false: a key or a conjunct they cannot read
+  bool parse_keys_and_conjuncts(FastSpec& fs) const {
+    if (lay_.nkeys < 1 || lay_.nkeys > 2 || filters_.size() > 4) return false;
+    fs.nkeys = lay_.nkeys; fs.nfilt = (int)filters_.size();
+    for (int k = 0; k < lay_.nkeys; k++) {
+      const ExprP& e = vm_outs_[lay_.key_out[k]];
+      if (e->kind != E_COLUMN || !int_phys(e->type) || lay_.key_nwords[k] != 1) return false;
+      const int s = prog_col_slot(e->col_index); if (s < 0 || s > 127) return false;
+      fs.key_col[k] = (int8_t)s; fs.key_phys[k] = phys_of(e->type);
+    }
+    for (size_t f = 0; f < filters_.size(); f++) {
+      const ExprP& p = filters_[f];
+      if (p->kind != E_BINARY || p->op < OP_EQ || p->op > OP_GE) return false;
+      ExprP l = strip_noop_casts(p->children[0]), r = strip_noop_casts(p->children[1]);
+      int op = p->op - OP_EQ;
+      if (l->kind == E_LITERAL && r->kind == E_COLUMN) { std::swap(l, r); static const int flip[] = {CMP_EQ, CMP_NE, CMP_GT, CMP_GE, CMP_LT, CMP_LE}; op = flip[op]; }
+      if (l->kind != E_COLUMN || r->kind != E_LITERAL || r->lit_null || !int_phys(l->type) || !int_phys(r->type)) return false;
+      const int s = prog_col_slot(l->col_index); if (s < 0 || s > 127) return false;
+      fs.filt[f].col = (int8_t)s; fs.filt[f].phys = phys_of(l->type); fs.filt[f].op = (uint8_t)op; fs.filt[f].lit = (long long)r->lit_lo;
+    }
+    merge_conjuncts(fs);
+    return true;
+  }
+
   void detect_fast(OpContext& cx) {
     fast_ok_ = false;
     if (cx.conf.force_generic_kernels) return;
-    if (lay_.nkeys < 1 || lay_.nkeys > 2 || lay_.nacc < 1 || lay_.nacc > 2 || filters_.size() > 4) return;
+    if (lay_.nacc < 1 || lay_.nacc > 2) return;
     FastSpec fs{};
-    fs.nkeys = lay_.nkeys; fs.nacc = lay_.nacc; fs.nfilt = (int)filters_.size();
-    for (int k = 0; k < lay_.nkeys; k++) {
-      const ExprP& e = vm_outs_[lay_.key_out[k]];
-      if (e->kind != E_COLUMN || !int_phys(e->type) || lay_.key_nwords[k] != 1) return;
-      const int s = prog_col_slot(e->col_index); if (s < 0 || s > 127) return;
-      fs.key_col[k] = (int8_t)s; fs.key_phys[k] = phys_of(e->type);
-    }
+    if (!parse_keys_and_conjuncts(fs)) return;
+    fs.nacc = lay_.nacc;
     for (int j = 0; j < lay_.nacc; j++) {
       const AccOp& a = lay_.acc[j];
       fs.acc[j].vbit = a.vbit; fs.acc[j].word = a.word; fs.acc[j].col = -1; fs.acc[j].phys = PH_I64;
@@ -726,18 +746,6 @@ class AggStage : public Stage {
       } else return;
     }
     if (lay_.nacc == 2 && lay_.acc[0].word / 4 != lay_.acc[1].word / 4) return;
-    for (size_t f = 0; f < filters_.size(); f++) {
-      const ExprP& p = filters_[f];
-      if (p->kind != E_BINARY || p->op < OP_EQ || p->op > OP_GE) return;
-      ExprP l = strip_noop_casts(p->children[0]), r = strip_noop_casts(p->children[1]);
-      int op = p->op - OP_EQ;
-      if (l->kind == E_LITERAL && r->kind == E_COLUMN) { std::swap(l, r); static const int flip[] = {CMP_EQ, CMP_NE, CMP_GT, CMP_GE, CMP_LT, CMP_LE}; op = flip[op]; }
-      if (l->kind != E_COLUMN || r->kind != E_LITERAL || r->lit_null || !int_phys(l->type) || !int_phys(r->type)) return;
-      const int s = prog_col_slot(l->col_index); if (s < 0 || s > 127) return;
-      fs.filt[f].col = (int8_t)s; fs.filt[f].phys = phys_of(l->type); fs.filt[f].op = (uint8_t)op; fs.filt[f].lit = (long long)r->lit_lo;
-    }
-    merge_conjuncts(fs);
-    { const char* e = getenv("B200Q_ROW_KERNELS"); fs.row_kernels = e && *e == '1'; }
     sink_ = DevMem::alloc((size_t)FAST_SINK_WARPS * 32, cx.stream, true);
     fs.sink = (unsigned long long*)sink_->ptr;
     fs_ = fs; fast_ok_ = true;
@@ -787,32 +795,15 @@ class AggStage : public Stage {
   void detect_wide(OpContext& cx) {
     wide_possible_ = false;
     if (cx.conf.force_generic_kernels || !cx.conf.agg_dense_keys) return;
-    if (lay_.nkeys < 1 || lay_.nkeys > 2 || lay_.nacc < 1 || lay_.nacc > 4 || filters_.size() > 4) return;
+    if (lay_.nacc < 1 || lay_.nacc > 4) return;
     TileAggSpec ts{};
-    ts.nkeys = lay_.nkeys; ts.nacc = lay_.nacc; ts.dec_word = 0xFF;
-    for (int k = 0; k < lay_.nkeys; k++) {
-      const ExprP& e = vm_outs_[lay_.key_out[k]];
-      if (e->kind != E_COLUMN || !int_phys(e->type) || lay_.key_nwords[k] != 1) return;
-      const int s = prog_col_slot(e->col_index); if (s < 0 || s > 127) return;
-      ts.key_col[k] = (int8_t)s; ts.key_phys[k] = phys_of(e->type);
+    {
+      FastSpec fs{};
+      if (!parse_keys_and_conjuncts(fs) || fs.nfcol < 0) return;
+      ts.nkeys = fs.nkeys; ts.nfcol = fs.nfcol; ts.filt_never = fs.filt_never;
+      for (int k = 0; k < 2; k++) { ts.key_col[k] = fs.key_col[k]; ts.key_phys[k] = fs.key_phys[k]; ts.frange[k] = fs.frange[k]; }
     }
-    {   // conjuncts -> intervals (shares merge_conjuncts with the FastSpec path)
-      FastSpec fs{}; fs.nfilt = (int)filters_.size();
-      for (size_t f = 0; f < filters_.size(); f++) {
-        const ExprP& p = filters_[f];
-        if (p->kind != E_BINARY || p->op < OP_EQ || p->op > OP_GE) return;
-        ExprP l = strip_noop_casts(p->children[0]), r = strip_noop_casts(p->children[1]);
-        int op = p->op - OP_EQ;
-        if (l->kind == E_LITERAL && r->kind == E_COLUMN) { std::swap(l, r); static const int flip[] = {CMP_EQ, CMP_NE, CMP_GT, CMP_GE, CMP_LT, CMP_LE}; op = flip[op]; }
-        if (l->kind != E_COLUMN || r->kind != E_LITERAL || r->lit_null || !int_phys(l->type) || !int_phys(r->type)) return;
-        const int s = prog_col_slot(l->col_index); if (s < 0 || s > 127) return;
-        fs.filt[f].col = (int8_t)s; fs.filt[f].phys = phys_of(l->type); fs.filt[f].op = (uint8_t)op; fs.filt[f].lit = (long long)r->lit_lo;
-      }
-      merge_conjuncts(fs);
-      if (fs.nfcol < 0) return;
-      ts.nfcol = fs.nfcol; ts.filt_never = fs.filt_never;
-      for (int c = 0; c < fs.nfcol; c++) { ts.frange[c].col = fs.frange[c].col; ts.frange[c].phys = fs.frange[c].phys; ts.frange[c].lo = fs.frange[c].lo; ts.frange[c].span = fs.frange[c].span; }
-    }
+    ts.nacc = lay_.nacc; ts.dec_word = 0xFF;
     // flavour
     bool any_f64 = false, any_min = false, any_int = false;
     for (int j = 0; j < lay_.nacc; j++) {
@@ -917,40 +908,55 @@ class AggStage : public Stage {
     ws_ = ts; wide_possible_ = true;
   }
 
-  // padded value range of the key columns from a sample of the first batch; false: not dense
-  bool sample_key_ranges(OpContext& cx, const ColTable& ct, int64_t n, int nkeys, const int8_t* key_col, const uint8_t* key_phys, int entry_words,
-                         long long (&base)[2], uint64_t (&span)[2]) {
+  // DENSE decision from the key ranges of (a sample of) the first batch.  The range kernel of every key (and, with
+  // probe_skew, the skew probe) are enqueued back to back and their results come back in ONE host round trip.  Each
+  // key's range is padded to [min - margin, max + margin]; false: the keys are too sparse for a table of entry_words
+  // words per entry, or it would exceed agg_max_table_bytes (stay on the hash table)
+  struct DenseRange { long long base[2] = {0, 0}; uint64_t span[2] = {1, 1}; uint64_t entries = 1; bool hot = false; };
+  bool dense_range(OpContext& cx, const ColTable& ct, int64_t n, int nkeys, const int8_t* key_col, const uint8_t* key_phys, int entry_words,
+                   bool probe_skew, DenseRange& dr) {
     const int64_t sample = std::min<int64_t>(n, 1 << 22);
-    base[0] = base[1] = 0; span[0] = span[1] = 1; long long nonnull = 0;
+    DevMemP d = DevMem::alloc(64, cx.stream);
+    { const long long init[8] = {INT64_MAX, INT64_MIN, 0, INT64_MAX, INT64_MIN, 0, 0, 0};
+      B200Q_CUDA(cudaMemcpyAsync(d->ptr, init, 64, cudaMemcpyHostToDevice, cx.stream)); }
+    for (int k = 0; k < nkeys; k++) cx.m.launches += launch_key_range(ct.col[key_col[k]], key_phys[k], sample, (long long*)d->ptr + 3 * k, cx.stream);
+    DevMemP hist;
+    if (probe_skew) {
+      hist = DevMem::alloc((65536 + 1) * 4, cx.stream, true);
+      DevCol kc[2] = {ct.col[key_col[0]], ct.col[key_col[nkeys == 2 ? 1 : 0]]};
+      cx.m.launches += launch_key_skew_probe(kc, key_phys, nkeys, sample, (unsigned*)hist->ptr, cx.stream);
+    }
+    long long hr[6] = {0}; unsigned mx = 0;
+    B200Q_CUDA(cudaMemcpyAsync(hr, d->ptr, 48, cudaMemcpyDeviceToHost, cx.stream));
+    if (probe_skew) B200Q_CUDA(cudaMemcpyAsync(&mx, (unsigned*)hist->ptr + 65536, 4, cudaMemcpyDeviceToHost, cx.stream));
+    B200Q_CUDA(cudaStreamSynchronize(cx.stream));
+    long long nonnull = 0;
     for (int k = 0; k < nkeys; k++) {
-      DevMemP d = DevMem::alloc(24, cx.stream);
-      const long long init[3] = {INT64_MAX, INT64_MIN, 0};
-      B200Q_CUDA(cudaMemcpyAsync(d->ptr, init, 24, cudaMemcpyHostToDevice, cx.stream));
-      cx.m.launches += launch_key_range(ct.col[key_col[k]], key_phys[k], sample, (long long*)d->ptr, cx.stream);
-      long long h[3];
-      B200Q_CUDA(cudaMemcpyAsync(h, d->ptr, 24, cudaMemcpyDeviceToHost, cx.stream));
-      B200Q_CUDA(cudaStreamSynchronize(cx.stream));
+      const long long* h = hr + 3 * k;                                     // {min, max, non-null rows}
       if (h[2] <= 0 || h[1] < h[0]) return false;
       const unsigned __int128 range = (unsigned __int128)((__int128)h[1] - (__int128)h[0]) + 1;
       if (range > ((uint64_t)1 << 26)) return false;
       const uint64_t r = (uint64_t)range, margin = r / 8 + std::min<uint64_t>(64, r / 2 + 1);
-      base[k] = h[0] > INT64_MIN + (long long)margin ? h[0] - (long long)margin : INT64_MIN;
-      span[k] = r + 2 * margin;
+      dr.base[k] = h[0] > INT64_MIN + (long long)margin ? h[0] - (long long)margin : INT64_MIN;
+      dr.span[k] = r + 2 * margin;
       nonnull = std::max(nonnull, h[2]);
     }
-    const unsigned __int128 entries = (unsigned __int128)span[0] * span[1];
+    const unsigned __int128 entries = (unsigned __int128)dr.span[0] * dr.span[1];
     const uint64_t budget = 8 * (uint64_t)std::max<int64_t>(std::max<int64_t>(nonnull, cx.conf.agg_initial_groups), 1 << 16);
     if (entries > budget || entries > ((uint64_t)1 << 26)) return false;               // sparse keys: stay on the hash table
     if (cx.conf.agg_max_table_bytes > 0 && entries * entry_words * 8 > (unsigned __int128)cx.conf.agg_max_table_bytes) return false;
+    dr.entries = (uint64_t)entries;
+    // do a few keys dominate the sample?  one hash bucket holds > 0.4 % of the rows
+    dr.hot = probe_skew && dr.entries * entry_words > 4096 && (uint64_t)mx * 256 > (uint64_t)sample;
     return true;
   }
 
   void decide_wide(OpContext& cx, const ColTable& ct, int64_t n) {
     dense_decided_ = true;
     if (!wide_possible_ || n == 0) { wide_possible_ = false; return; }
-    long long base[2]; uint64_t span[2];
-    if (!sample_key_ranges(cx, ct, n, ws_.nkeys, ws_.key_col, ws_.key_phys, ws_.G, base, span)) { wide_possible_ = false; return; }
-    ws_.dense_base = base[0]; ws_.dense_cap0 = span[0]; ws_.dense_base1 = base[1]; ws_.dense_r1 = span[1]; ws_.dense_cap = span[0] * span[1];
+    DenseRange dr;
+    if (!dense_range(cx, ct, n, ws_.nkeys, ws_.key_col, ws_.key_phys, ws_.G, false, dr)) { wide_possible_ = false; return; }
+    ws_.dense_base = dr.base[0]; ws_.dense_cap0 = dr.span[0]; ws_.dense_base1 = dr.base[1]; ws_.dense_r1 = dr.span[1]; ws_.dense_cap = dr.entries;
     dense_tab_ = DevMem::alloc((size_t)ws_.dense_cap * ws_.G * 8, cx.stream);
     ws_.dense_tab = (unsigned long long*)dense_tab_->ptr;
     cx.m.launches += launch_tile_wide_init(ws_, cx.stream);
@@ -988,53 +994,19 @@ class AggStage : public Stage {
     return true;
   }
 
-  // decide DENSE mode from the key range of (a sample of) the first batch
+  // decide DENSE mode from the key range of (a sample of) the first batch; dense_layout() already ran in detect_fast
   void decide_dense(OpContext& cx, const ColTable& ct, int64_t n) {
     dense_decided_ = true;
     if (!fast_ok_ || !dense_possible_ || n == 0) return;
-    const int64_t sample = std::min<int64_t>(n, 1 << 22);
-    // padded value range of every key column: [min - margin, max + margin] of the sample
-    long long base[2] = {0, 0}; uint64_t span[2] = {1, 1}; long long nonnull = 0;
-    // ONE host round trip for the whole decision: the range kernels of every key and the skew probe are enqueued back to back, their results
-    // come back together
-    DevMemP d = DevMem::alloc(64, cx.stream);
-    { const long long init[8] = {INT64_MAX, INT64_MIN, 0, INT64_MAX, INT64_MIN, 0, 0, 0};
-      B200Q_CUDA(cudaMemcpyAsync(d->ptr, init, 64, cudaMemcpyHostToDevice, cx.stream)); }
-    for (int k = 0; k < fs_.nkeys; k++) cx.m.launches += launch_key_range(ct.col[fs_.key_col[k]], fs_.key_phys[k], sample, (long long*)d->ptr + 3 * k, cx.stream);
-    DevMemP hist;
-    const bool probe_skew = cx.conf.agg_hot_key_cache != 0;
-    if (probe_skew) {
-      hist = DevMem::alloc((65536 + 1) * 4, cx.stream, true);
-      DevCol kc[2] = {ct.col[fs_.key_col[0]], ct.col[fs_.key_col[fs_.nkeys == 2 ? 1 : 0]]};
-      cx.m.launches += launch_key_skew_probe(kc, fs_.key_phys, fs_.nkeys, sample, (unsigned*)hist->ptr, cx.stream);
-    }
-    long long hr[8] = {0}; unsigned mx = 0;
-    B200Q_CUDA(cudaMemcpyAsync(hr, d->ptr, 48, cudaMemcpyDeviceToHost, cx.stream));
-    if (probe_skew) B200Q_CUDA(cudaMemcpyAsync(&mx, (unsigned*)hist->ptr + 65536, 4, cudaMemcpyDeviceToHost, cx.stream));
-    B200Q_CUDA(cudaStreamSynchronize(cx.stream));
-    for (int k = 0; k < fs_.nkeys; k++) {
-      const long long* h = hr + 3 * k;
-      if (h[2] <= 0 || h[1] < h[0]) return;
-      const unsigned __int128 range = (unsigned __int128)((__int128)h[1] - (__int128)h[0]) + 1;
-      if (range > ((uint64_t)1 << 26)) return;
-      const uint64_t r = (uint64_t)range, margin = r / 8 + std::min<uint64_t>(64, r / 2 + 1);
-      base[k] = h[0] > INT64_MIN + (long long)margin ? h[0] - (long long)margin : INT64_MIN;
-      span[k] = r + 2 * margin;
-      nonnull = std::max(nonnull, h[2]);
-    }
-    const unsigned __int128 entries = (unsigned __int128)span[0] * span[1];
-    const uint64_t budget = 8 * (uint64_t)std::max<int64_t>(std::max<int64_t>(nonnull, cx.conf.agg_initial_groups), 1 << 16);
-    if (entries > budget || entries > ((uint64_t)1 << 26)) return;             // sparse keys: stay on the hash table
-    fs_.dense_base = base[0]; fs_.dense_cap0 = span[0];
-    fs_.dense_base1 = base[1]; fs_.dense_r1 = span[1];
-    fs_.dense_cap = (uint64_t)entries;
-    dense_layout();
-    if (cx.conf.agg_max_table_bytes > 0 && (unsigned __int128)fs_.dense_cap * fs_.dense_stride * 8 > (unsigned __int128)cx.conf.agg_max_table_bytes) return;   // over budget: stay hashed
+    DenseRange dr;
+    if (!dense_range(cx, ct, n, fs_.nkeys, fs_.key_col, fs_.key_phys, fs_.dense_stride, cx.conf.agg_hot_key_cache != 0, dr)) return;
+    fs_.dense_base = dr.base[0]; fs_.dense_cap0 = dr.span[0];
+    fs_.dense_base1 = dr.base[1]; fs_.dense_r1 = dr.span[1];
+    fs_.dense_cap = dr.entries;
     dense_tab_ = DevMem::alloc((size_t)fs_.dense_cap * fs_.dense_stride * 8, cx.stream, true);
     fs_.dense_tab = (unsigned long long*)dense_tab_->ptr;
     fs_.dense = 1;
-    if (probe_skew && fs_.dense_cap * fs_.dense_stride > 4096)                 // do a few keys dominate the sample?  one hash bucket holds > 0.4 % of the rows
-      fs_.hot_cache = (uint64_t)mx * 256 > (uint64_t)sample ? 1 : 0;
+    fs_.hot_cache = dr.hot ? 1 : 0;
   }
 
   // LEAN kernels: every referenced column is a non-null, 32-byte aligned int64 column
@@ -1106,11 +1078,9 @@ class AggStage : public Stage {
 
   // probe chains cost one dependent L2 round trip per extra slot: the table is kept at most half full (measured on
   // M1-hash: load 0.3 -> 6.7e10 rows/s, load 0.6 -> 5.6e10; only the sectors holding occupied slots are L2-resident)
-  // experiment knobs (percent): slots per expected group, load limit
-  static double cap_factor() { static const double f = getenv("B200Q_AGG_CAP_PCT") ? atof(getenv("B200Q_AGG_CAP_PCT")) / 100.0 : 3.0; return f; }
+  static constexpr double AGG_SLOTS_PER_GROUP = 3.0, AGG_LOAD_LIMIT = 0.5;
   static uint64_t load_limit(uint64_t cap) {
-    static const double l = getenv("B200Q_AGG_LOAD_PCT") ? atof(getenv("B200Q_AGG_LOAD_PCT")) / 100.0 : 0.5;
-    const uint64_t lim = (uint64_t)((double)cap * l);
+    const uint64_t lim = (uint64_t)((double)cap * AGG_LOAD_LIMIT);
     return cap > (1ULL << 19) ? std::min<uint64_t>(lim, cap - (1ULL << 19)) : lim;      // slack above the limit > the concurrent-insert overshoot bound (resident threads)
   }
 

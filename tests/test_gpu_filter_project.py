@@ -165,9 +165,8 @@ def test_lean_project_only_and_filter_only():
 
 @pytest.mark.parametrize("n", [1 << 20, 3_000_037])
 def test_lean_large_batch_forms(n):
-    """batches of >= 2^20 rows take the order-free count / scan / apply form (or, with B200Q_FILTER_TMA=1, the TMA-staged single pass:
-    cp.async.bulk tiles + decoupled look-back over a fully resident grid — bit-exact but not faster, see kernels.cu): ragged last
-    tile, 3 input columns, conjuncts on two of them, every selectivity regime inside one batch (sorted run + random part)"""
+    """batches of >= 2^20 rows take the order-free count / scan / apply form: ragged last tile, 3 input columns, conjuncts on
+    two of them, every selectivity regime inside one batch (sorted run + random part)"""
     rng = np.random.default_rng(n)
     a = rng.integers(0, 1000, n, dtype=np.int64); a[: n // 4] = np.sort(a[: n // 4])
     b = rng.integers(-2**31, 2**31, n, dtype=np.int64)
@@ -182,8 +181,8 @@ def test_lean_large_batch_forms(n):
 
 @pytest.mark.parametrize("ncols", [1, 2, 4])
 def test_lean_large_batch_column_counts_and_unaligned_slices(ncols):
-    """1 / 2 / 4 input columns; a batch that starts one row into its buffers is 8- but not 16-byte aligned (the bulk copies of the
-    opt-in TMA form cannot read it and fall back to the two-pass form): same rows either way"""
+    """1 / 2 / 4 input columns; a batch that starts one row into its buffers is 8- but not 16-byte aligned: the two-pass form
+    gives the same rows either way"""
     n = (1 << 20) + 4321
     rng = np.random.default_rng(ncols)
     cols = [rng.integers(0, 1000, n + 1, dtype=np.int64) for _ in range(ncols)]
