@@ -764,7 +764,7 @@ int launch_agg_fast_update(const ColTable& cols, const FastSpec& fs, const AggLa
 #undef B200Q_LD
     return 1;
   }
-  if (dg && fs.nfcol >= 0) {                                    // filters / two keys / typed inputs: 128-row tiles, 4 rows per lane (kernels_tile.cu)
+  if (dg && fs.nfcol >= 0) {                                    // filters / two keys / typed inputs: 128-row tiles, filter first (kernels_tile.cu)
     if (fs.filt_never) return 0;
     return launch_agg_tile_dense(cols, fs, lay, tab, row_begin, n, s);
   }

@@ -4,16 +4,22 @@
 // Why: the one-row-per-lane kernels of kernels_fast.cu issue one 8-byte (or narrower) load per row per column plus one
 // validity-byte load per row, re-read a filter column once per conjunct, and run G shuffle + RED steps per 32 rows
 // whether or not the rows survived the filter.
-// Here a warp owns a TILE of 128 consecutive rows and every lane 4 consecutive rows of it:
-//   * one 32-byte run per column per lane (two 128-bit loads for int64, one 128-bit for int32, 64/32-bit for int16/int8) and ONE
-//     validity nibble per column per lane (a 32-lane load covers 128 validity bits);
+// Here a warp owns a TILE of 128 consecutive rows and lane l holds rows l, l + 32, l + 64 and l + 96 of it:
+//   * one warp-wide load reads 32 consecutive rows of a column, i.e. whole 32-byte sectors at every width (256 bytes of
+//     an int64 column, 512 of a decimal128, 32 of an int8); a validity bitmap is read as the byte that holds the lane's
+//     bit (32 lanes: one 4-byte run per 32 rows);
+//   * FILTER FIRST: with fused conjuncts the filter columns are read in full, and the key and argument columns (values and
+//     validity) only for the rows that pass — a predicated per-row load, so a sector without a surviving row is never
+//     requested (DESIGN §3.1 measures what that saves); a filter column that is also a key or argument is read once;
+//   * the filter columns of the warp's NEXT tile are in flight while the current tile is compacted and reduced;
 //   * the conjuncts on one column are merged on the host into one closed interval [lo, hi] (FilterExec conjuncts are
 //     pre-split `col cmp literal` terms, NativeFilterBase.scala:66-87), tested with one subtract + one unsigned compare;
 //   * rows that survive are COMPACTED into a per-warp shared-memory queue (ballot + popc, no atomics), and the dense
 //     table is updated from the queue G lanes per entry: one RED instruction updates the G words of 32/G rows, so a
 //     selectivity of 0.2 costs 0.2 x the RED issue slots and sector operations instead of 1.0 x.
 // Semantics are those of agg_dense_row_kernel (same table, same entry layout, same fall-back of NULL / out-of-range
-// keys to the hashed slots, same deferred-row protocol), so the emit / grow / replay code is shared.
+// keys to the hashed slots, same deferred-row protocol: a deferred entry is the row's launch-relative index), so the
+// emit / grow / replay code is shared.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -30,85 +36,119 @@ constexpr int TL_BLOCK = 256, TL_WARPS = TL_BLOCK / 32, TL_ROWS = 128;
 __device__ __forceinline__ uint64_t tl_policy_evict_first() {
   uint64_t pol; asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol)); return pol;
 }
-// 4 consecutive int64 as two 128-bit loads (the widest a thread can issue on sm_90); p is 16-byte aligned
-__device__ __forceinline__ void tl_ld_v4b64(const long long* p, uint64_t pol, long long (&v)[4]) {
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0,%1}, [%4], %5;\n\tld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%2,%3}, [%4+16], %5;"
-               : "=l"(v[0]), "=l"(v[1]), "=l"(v[2]), "=l"(v[3]) : "l"(p), "l"(pol));
+// predicated streaming loads: nothing is requested when `on` is 0 (the destination keeps its value)
+__device__ __forceinline__ void tl_ld_b64(const long long* p, unsigned on, uint64_t pol, long long& v) {
+  asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q ld.global.nc.L1::no_allocate.L2::cache_hint.b64 %0, [%1], %3;\n\t}"
+               : "+l"(v) : "l"(p), "r"(on), "l"(pol));
 }
-__device__ __forceinline__ long long tl_ld_b64(const long long* p, uint64_t pol) {
-  long long v; asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.b64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol)); return v;
+__device__ __forceinline__ void tl_ld_v2b64(const long long* p, unsigned on, uint64_t pol, long long& a, long long& b) {   // p is 16-byte aligned
+  asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %3, 0;\n\t@q ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0,%1}, [%2], %4;\n\t}"
+               : "+l"(a), "+l"(b) : "l"(p), "r"(on), "l"(pol));
 }
-__device__ __forceinline__ void tl_ld_v4b32(const int* p, uint64_t pol, int (&v)[4]) {
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.b32 {%0,%1,%2,%3}, [%4], %5;" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "l"(p), "l"(pol));
-}
-__device__ __forceinline__ void tl_ld_v2b32(const int* p, uint64_t pol, int (&v)[2]) {
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b32 {%0,%1}, [%2], %3;" : "=r"(v[0]), "=r"(v[1]) : "l"(p), "l"(pol));
-}
-__device__ __forceinline__ int tl_ld_b32(const int* p, uint64_t pol) {
-  int v; asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.b32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol)); return v;
+__device__ __forceinline__ void tl_ld_b32(const int* p, unsigned on, uint64_t pol, int& v) {
+  asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q ld.global.nc.L1::no_allocate.L2::cache_hint.b32 %0, [%1], %3;\n\t}"
+               : "+r"(v) : "l"(p), "r"(on), "l"(pol));
 }
 
-// 4 bits starting at bit `bi` of a bitmap; bits of rows >= nrow are not touched in memory
-__device__ __forceinline__ unsigned tl_nibble(const uint8_t* bits, unsigned long long bi, int nrow) {
-  const unsigned sh = (unsigned)bi & 7u;
-  unsigned w = __ldg(bits + (bi >> 3));
-  if (sh + (unsigned)nrow > 8u) w |= (unsigned)__ldg(bits + (bi >> 3) + 1) << 8;
-  return (w >> sh) & 0xFu;
+// bit j set: row l + 32 j of the tile (launch-relative `rel` of j = 0) lies below n
+__device__ __forceinline__ unsigned tl_rows_in(long long rel, long long n) {
+  const long long left = n - rel;
+  return left > 96 ? 0xFu : left > 64 ? 0x7u : left > 32 ? 0x3u : left > 0 ? 0x1u : 0u;
 }
 
-// the 4 rows [row0, row0 + 4) of one column as sign-extended int64 + their validity bits; rows >= nrow read as 0 / invalid.
-// `want_values` = false: only the validity (COUNT(col) never looks at the values).
-__device__ __forceinline__ void tl_load4(const DevCol& c, int phys, long long row0, int nrow, bool want_values, uint64_t pol, long long (&v)[4], unsigned& valid) {
-  valid = (1u << nrow) - 1u;
-  if (c.validity && nrow > 0) valid &= tl_nibble(c.validity, (unsigned long long)row0 + c.bit_offset, nrow);
+// rows r0 + 32 j (j = 0..3) of one column as sign-extended int64 + their validity bits, for the rows whose bit is set in `ld`;
+// the other rows read as 0 / invalid and are not touched in memory.  `want_values` = false: only the validity (COUNT(col)).
+__device__ __forceinline__ void tl_load(const DevCol& c, int phys, long long r0, unsigned ld, bool want_values, uint64_t pol, long long (&v)[4], unsigned& valid) {
+  valid = ld;
+  if (c.validity) {
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const unsigned long long bi = (unsigned long long)(r0 + 32 * j) + c.bit_offset;
+      const unsigned b = ((ld >> j) & 1u) ? __ldg(c.validity + (bi >> 3)) : 0u;
+      valid &= ~((((b >> (bi & 7)) & 1u) ^ 1u) << j);
+    }
+  }
 #pragma unroll
   for (int j = 0; j < 4; j++) v[j] = 0;
-  if (!want_values || nrow <= 0) return;
+  if (!want_values) return;
   switch (phys) {
     case PH_I64: {
-      const long long* p = (const long long*)c.values + row0;
-      if (nrow == 4 && ((uintptr_t)p & 15) == 0) tl_ld_v4b64(p, pol, v);
-      else {
+      const long long* p = (const long long*)c.values + r0;
 #pragma unroll
-        for (int j = 0; j < 4; j++) if (j < nrow) v[j] = tl_ld_b64(p + j, pol);
-      }
+      for (int j = 0; j < 4; j++) tl_ld_b64(p + 32 * j, (ld >> j) & 1u, pol, v[j]);
       break;
     }
     case PH_I32: {
-      const int* p = (const int*)c.values + row0;
-      if (nrow == 4 && ((uintptr_t)p & 15) == 0) { int t[4]; tl_ld_v4b32(p, pol, t); v[0] = t[0]; v[1] = t[1]; v[2] = t[2]; v[3] = t[3]; }
-      else {
+      const int* p = (const int*)c.values + r0;
 #pragma unroll
-        for (int j = 0; j < 4; j++) if (j < nrow) v[j] = tl_ld_b32(p + j, pol);
-      }
+      for (int j = 0; j < 4; j++) { int t = 0; tl_ld_b32(p + 32 * j, (ld >> j) & 1u, pol, t); v[j] = t; }
       break;
     }
     case PH_I16: {
-      const int16_t* p = (const int16_t*)c.values + row0;
-      if (nrow == 4 && ((uintptr_t)p & 7) == 0) { int t[2]; tl_ld_v2b32((const int*)p, pol, t); v[0] = (int16_t)t[0]; v[1] = (int16_t)(t[0] >> 16); v[2] = (int16_t)t[1]; v[3] = (int16_t)(t[1] >> 16); }
-      else {
+      const int16_t* p = (const int16_t*)c.values + r0;
 #pragma unroll
-        for (int j = 0; j < 4; j++) if (j < nrow) v[j] = __ldg(p + j);
-      }
+      for (int j = 0; j < 4; j++) v[j] = ((ld >> j) & 1u) ? __ldg(p + 32 * j) : 0;
       break;
     }
     case PH_I8: {
-      const int8_t* p = (const int8_t*)c.values + row0;
-      if (nrow == 4 && ((uintptr_t)p & 3) == 0) { const int t = tl_ld_b32((const int*)p, pol); v[0] = (int8_t)t; v[1] = (int8_t)(t >> 8); v[2] = (int8_t)(t >> 16); v[3] = (int8_t)(t >> 24); }
-      else {
+      const int8_t* p = (const int8_t*)c.values + r0;
 #pragma unroll
-        for (int j = 0; j < 4; j++) if (j < nrow) v[j] = __ldg(p + j);
-      }
+      for (int j = 0; j < 4; j++) v[j] = ((ld >> j) & 1u) ? __ldg(p + 32 * j) : 0;
       break;
     }
     default: {                                                    // PH_BOOL: bit-packed values
-      const unsigned b = tl_nibble((const uint8_t*)c.values, (unsigned long long)row0 + c.bit_offset, nrow);
 #pragma unroll
-      for (int j = 0; j < 4; j++) v[j] = (b >> j) & 1u;
+      for (int j = 0; j < 4; j++) {
+        const unsigned long long bi = (unsigned long long)(r0 + 32 * j) + c.bit_offset;
+        v[j] = ((ld >> j) & 1u) ? (__ldg((const uint8_t*)c.values + (bi >> 3)) >> (bi & 7)) & 1u : 0u;
+      }
       break;
     }
   }
 }
+
+// the filter columns of the tile whose lane-0 row is `rel` (all its rows below n), and the rows that pass every interval
+template <int NF>
+__device__ __forceinline__ void tl_load_filters(const ColTable& cols, const FilterInterval (&fr)[2], long long row_begin, long long rel, long long n, uint64_t pol,
+                                                long long (&f)[NF > 0 ? NF : 1][4], unsigned (&fv)[NF > 0 ? NF : 1]) {
+  const unsigned in = tl_rows_in(rel, n);
+#pragma unroll
+  for (int c = 0; c < NF; c++) tl_load(cols.col[fr[c].col], fr[c].phys, row_begin + rel, in, true, pol, f[c], fv[c]);
+}
+template <int NF>
+__device__ __forceinline__ unsigned tl_pass(const FilterInterval (&fr)[2], const long long (&f)[NF > 0 ? NF : 1][4], const unsigned (&fv)[NF > 0 ? NF : 1], unsigned in) {
+  unsigned alive = in;
+#pragma unroll
+  for (int c = 0; c < NF; c++) {
+    unsigned pass = 0;
+#pragma unroll
+    for (int j = 0; j < 4; j++) pass |= (unsigned)((unsigned long long)(f[c][j] - fr[c].lo) <= fr[c].span) << j;
+    alive &= pass & fv[c];                                          // NULL -> row dropped (cached_exprs_evaluator.rs:518-520)
+  }
+  return alive;
+}
+// a key / argument column that is also filter column c >= 0 is taken from the filter registers instead of being read again
+template <int NF>
+__device__ __forceinline__ int tl_filter_of(const FilterInterval (&fr)[2], int col) {
+  return NF > 0 && fr[0].col == col ? 0 : (NF > 1 && fr[NF > 1 ? 1 : 0].col == col ? 1 : -1);
+}
+template <int NF>
+__device__ __forceinline__ void tl_column(const ColTable& cols, const FilterInterval (&fr)[2], const long long (&f)[NF > 0 ? NF : 1][4], const unsigned (&fv)[NF > 0 ? NF : 1],
+                                          int col, int phys, long long r0, unsigned ld, bool want_values, uint64_t pol, long long (&v)[4], unsigned& valid) {
+  const int fc = tl_filter_of<NF>(fr, col);
+  tl_load(cols.col[col], phys, r0, fc < 0 ? ld : 0u, want_values, pol, v, valid);
+  if (fc >= 0) {
+#pragma unroll
+    for (int j = 0; j < 4; j++) v[j] = fc == 0 ? f[0][j] : f[NF > 1 ? 1 : 0][j];
+    valid = (fc == 0 ? fv[0] : fv[NF > 1 ? 1 : 0]) & ld;
+  }
+}
+
+// resident CTAs per SM the register allocation must allow: 4 (64 registers a thread) for the instances that fit them without
+// a spill, among them the q1 shape <2,1,2,1>; 3 (80 registers) for the one-key wide instances without a filter, which ptxas
+// otherwise squeezes into 64 registers with spills; no bound for the others.  tile_grid sizes every grid from the result.
+#define TD_MIN_CTAS(NK, NACC, NF) ((NACC == 1 ? (NK == 1 || NF < 2) : (NK == 1 && NF == 0)) ? 4 : 1)
+#define TW_MIN_CTAS(NK, NF) ((NK == 1 && NF == 0) ? 3 : 1)
 
 enum { TW_ZERO = 0, TW_ONE, TW_ADD0, TW_ADD1, TW_VALID0, TW_VALID1 };     // what an entry word accumulates
 
@@ -118,7 +158,7 @@ struct TileQueue {                                                  // per warp:
 };
 
 template <int NK, int NACC, int G, int NF>
-__global__ void __launch_bounds__(TL_BLOCK) agg_tile_dense_kernel(const ColTable cols, const FastSpec fs, const AggLayout lay, const AggTable tab,
+__global__ void __launch_bounds__(TL_BLOCK, TD_MIN_CTAS(NK, NACC, NF)) agg_tile_dense_kernel(const ColTable cols, const FastSpec fs, const AggLayout lay, const AggTable tab,
                                                                   long long row_begin, long long n) {
   constexpr unsigned IDX_MASK = 0x0FFFFFFFu;                        // dense_cap <= 2^26
   constexpr unsigned FULL = 0xffffffffu;
@@ -145,30 +185,22 @@ __global__ void __launch_bounds__(TL_BLOCK) agg_tile_dense_kernel(const ColTable
   unsigned long long* const sink = fs.sink + ((gwarp & (FAST_SINK_WARPS - 1)) << 2) + (lane & 3);
   const uint64_t pol = tl_policy_evict_first();
 
+  long long f[NF > 0 ? NF : 1][4]; unsigned fv[NF > 0 ? NF : 1];
+  tl_load_filters<NF>(cols, fs.frange, row_begin, gwarp * TL_ROWS + lane, n, pol, f, fv);
   for (long long tile = gwarp; tile < ntiles; tile += nwarps) {
-    const long long rel0 = tile * TL_ROWS + lane * 4, row0 = row_begin + rel0;
-    const int nrow = (int)(n - rel0 >= 4 ? 4 : (n - rel0 > 0 ? n - rel0 : 0));
-    // ---- loads: everything this tile needs is in flight before the first use
-    long long f[NF > 0 ? NF : 1][4]; unsigned fv[NF > 0 ? NF : 1];
+    const long long rel0 = tile * TL_ROWS + lane, row0 = row_begin + rel0;
+    // ---- filter first: the key and argument columns are read only for the rows that pass
+    const unsigned alive = tl_pass<NF>(fs.frange, f, fv, tl_rows_in(rel0, n));
     long long k0[4], k1[4], a0[4], a1[4]; unsigned kv0, kv1 = 0xF, av0 = 0xF, av1 = 0xF;
-#pragma unroll
-    for (int c = 0; c < NF; c++) tl_load4(cols.col[fs.frange[c].col], fs.frange[c].phys, row0, nrow, true, pol, f[c], fv[c]);
-    tl_load4(cols.col[fs.key_col[0]], fs.key_phys[0], row0, nrow, true, pol, k0, kv0);
-    if (NK == 2) tl_load4(cols.col[fs.key_col[1]], fs.key_phys[1], row0, nrow, true, pol, k1, kv1);
+    tl_column<NF>(cols, fs.frange, f, fv, fs.key_col[0], fs.key_phys[0], row0, alive, true, pol, k0, kv0);
+    if (NK == 2) tl_column<NF>(cols, fs.frange, f, fv, fs.key_col[1], fs.key_phys[1], row0, alive, true, pol, k1, kv1);
     else { k1[0] = k1[1] = k1[2] = k1[3] = 0; }
-    if (fs.acc[0].col >= 0) tl_load4(cols.col[fs.acc[0].col], fs.acc[0].phys, row0, nrow, add0, pol, a0, av0);
+    if (fs.acc[0].col >= 0) tl_column<NF>(cols, fs.frange, f, fv, fs.acc[0].col, fs.acc[0].phys, row0, alive, add0, pol, a0, av0);
     else { a0[0] = a0[1] = a0[2] = a0[3] = 0; }
-    if (NACC == 2 && fs.acc[1].col >= 0) tl_load4(cols.col[fs.acc[1].col], fs.acc[1].phys, row0, nrow, add1, pol, a1, av1);
+    if (NACC == 2 && fs.acc[1].col >= 0) tl_column<NF>(cols, fs.frange, f, fv, fs.acc[1].col, fs.acc[1].phys, row0, alive, add1, pol, a1, av1);
     else { a1[0] = a1[1] = a1[2] = a1[3] = 0; }
-    // ---- fused FilterExec conjuncts: NULL -> row dropped (cached_exprs_evaluator.rs:518-520)
-    unsigned alive = (1u << nrow) - 1u;
-#pragma unroll
-    for (int c = 0; c < NF; c++) {
-      unsigned pass = 0;
-#pragma unroll
-      for (int j = 0; j < 4; j++) pass |= (unsigned)((unsigned long long)(f[c][j] - fs.frange[c].lo) <= fs.frange[c].span) << j;
-      alive &= pass & fv[c];
-    }
+    // ---- the next tile's filter columns are in flight while this one is compacted and reduced
+    tl_load_filters<NF>(cols, fs.frange, row_begin, rel0 + nwarps * TL_ROWS, n, pol, f, fv);
     // ---- compaction of the surviving rows with an in-range, non-NULL key
     const unsigned knull = (~kv0 | (NK == 2 ? ~kv1 : 0u)) & 0xFu;
     int total = 0; unsigned fb = 0;
@@ -210,7 +242,7 @@ __global__ void __launch_bounds__(TL_BLOCK) agg_tile_dense_kernel(const ColTable
           uint64_t kw[2] = {(kn & 1u) ? 0ULL : (uint64_t)k0[j], (NK == 2 && !(kn & 2u)) ? (uint64_t)k1[j] : 0ULL};
           unsigned fl = 0;
           const uint64_t si = agg_find_or_insert(lay, tab, kw, kn, agg_hash2(kw[0], kw[1], kn), &fl, &inserted);
-          if (si == AGG_NO_SLOT) { const unsigned long long at = atomicAdd(tab.counters + 1, 1ULL); tab.deferred[at] = (uint32_t)(rel0 + j); }
+          if (si == AGG_NO_SLOT) { const unsigned long long at = atomicAdd(tab.counters + 1, 1ULL); tab.deferred[at] = (uint32_t)(rel0 + 32 * j); }
           else {
             unsigned long long* const p = tab.accs + si * (uint64_t)lay.astride;
             unsigned long long* const ke = tab.keys + si * (uint64_t)lay.kstride;
@@ -225,17 +257,20 @@ __global__ void __launch_bounds__(TL_BLOCK) agg_tile_dense_kernel(const ColTable
   }
 }
 
-static int tile_grid(int64_t ntiles, int ctas_per_sm) {
-  int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int64_t want = (ntiles + TL_WARPS - 1) / TL_WARPS, cap = (int64_t)sms * ctas_per_sm;      // persistent grid: a multiple of the SM count
-  return (int)std::max<int64_t>(1, std::min(want, cap));
+// persistent grid of 256-thread CTAs: one full wave of `kernel` (the CTAs per SM its registers and shared memory allow x
+// the SM count), or `units` CTAs when there is less work than that
+template <class K>
+static int tile_grid(K kernel, int64_t units) {
+  int dev = 0, sms = 132, per_sm = 1; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, TL_BLOCK, 0) != cudaSuccess || per_sm < 1) per_sm = 1;
+  return (int)std::max<int64_t>(1, std::min<int64_t>(units, (int64_t)sms * per_sm));
 }
 
 int launch_agg_tile_dense(const ColTable& cols, const FastSpec& fs, const AggLayout& lay, const AggTable& tab, int64_t row_begin, int64_t n, cudaStream_t s) {
   if (n <= 0) return 0;
-  const int g = tile_grid((n + TL_ROWS - 1) / TL_ROWS, 4);
+  const int64_t units = ((n + TL_ROWS - 1) / TL_ROWS + TL_WARPS - 1) / TL_WARPS;
   const int G = fs.dense_stride;
-#define B200Q_TD(NK, NACC, G_, NF) agg_tile_dense_kernel<NK, NACC, G_, NF><<<g, TL_BLOCK, 0, s>>>(cols, fs, lay, tab, row_begin, n)
+#define B200Q_TD(NK, NACC, G_, NF) do { auto k_ = agg_tile_dense_kernel<NK, NACC, G_, NF>; k_<<<tile_grid(k_, units), TL_BLOCK, 0, s>>>(cols, fs, lay, tab, row_begin, n); } while (0)
 #define B200Q_TD_NF(NK, NACC, G_) do { if (fs.nfcol == 0) B200Q_TD(NK, NACC, G_, 0); else if (fs.nfcol == 1) B200Q_TD(NK, NACC, G_, 1); else B200Q_TD(NK, NACC, G_, 2); } while (0)
 #define B200Q_TD_G(NK, NACC) do { if (G == 2) B200Q_TD_NF(NK, NACC, 2); else B200Q_TD_NF(NK, NACC, 4); } while (0)
   if (fs.nkeys == 1) { if (fs.nacc == 2) B200Q_TD_G(1, 2); else B200Q_TD_G(1, 1); }
@@ -256,20 +291,17 @@ template <int FLAV> __device__ __forceinline__ void tw_red(unsigned long long* p
 }
 template <int FLAV> __device__ __forceinline__ unsigned long long tw_noop() { return FLAV == TF_MIN_S64 ? 0x7FFFFFFFFFFFFFFFULL : 0ULL; }
 
-// the 4 rows of one decimal128 column: low and high words (four 128-bit loads per lane)
-__device__ __forceinline__ void tl_load4_dec(const DevCol& c, long long row0, int nrow, uint64_t pol, long long (&lo)[4], long long (&hi)[4], unsigned& valid) {
-  valid = (1u << nrow) - 1u;
-  if (c.validity && nrow > 0) valid &= tl_nibble(c.validity, (unsigned long long)row0 + c.bit_offset, nrow);
+// rows r0 + 32 j of one decimal128 column (bit j of `ld`): low and high words, one 128-bit load per row when the column is
+// 16-byte aligned (an Arrow slice of an 8-byte aligned buffer may not be: two 64-bit loads)
+__device__ __forceinline__ void tl_load_dec(const DevCol& c, long long r0, unsigned ld, uint64_t pol, long long (&lo)[4], long long (&hi)[4], unsigned& valid) {
+  tl_load(c, PH_I64, r0, ld, false, pol, lo, valid);
+  const long long* p = (const long long*)c.values + 2 * r0;
+  const bool a16 = ((uintptr_t)c.values & 15) == 0;
 #pragma unroll
-  for (int j = 0; j < 4; j++) { lo[j] = 0; hi[j] = 0; }
-  if (nrow <= 0) return;
-  const long long* p = (const long long*)c.values + 2 * row0;
-  if (nrow == 4 && ((uintptr_t)p & 15) == 0) {
-    long long a[4], b[4]; tl_ld_v4b64(p, pol, a); tl_ld_v4b64(p + 4, pol, b);
-    lo[0] = a[0]; hi[0] = a[1]; lo[1] = a[2]; hi[1] = a[3]; lo[2] = b[0]; hi[2] = b[1]; lo[3] = b[2]; hi[3] = b[3];
-  } else {
-#pragma unroll
-    for (int j = 0; j < 4; j++) if (j < nrow) { lo[j] = tl_ld_b64(p + 2 * j, pol); hi[j] = tl_ld_b64(p + 2 * j + 1, pol); }
+  for (int j = 0; j < 4; j++) {
+    lo[j] = 0; hi[j] = 0;
+    if (a16) tl_ld_v2b64(p + 64 * j, (ld >> j) & 1u, pol, lo[j], hi[j]);
+    else { tl_ld_b64(p + 64 * j, (ld >> j) & 1u, pol, lo[j]); tl_ld_b64(p + 64 * j + 1, (ld >> j) & 1u, pol, hi[j]); }
   }
 }
 
@@ -302,7 +334,7 @@ __device__ __forceinline__ void tw_slot_update(const AggLayout& lay, const TileA
 }
 
 template <int NK, int NF, int G, int FLAV>
-__global__ void __launch_bounds__(TL_BLOCK) agg_tile_wide_kernel(const ColTable cols, const TileAggSpec ts, const AggLayout lay, const AggTable tab, long long row_begin, long long n) {
+__global__ void __launch_bounds__(TL_BLOCK, TW_MIN_CTAS(NK, NF)) agg_tile_wide_kernel(const ColTable cols, const TileAggSpec ts, const AggLayout lay, const AggTable tab, long long row_begin, long long n) {
   constexpr unsigned IDX_MASK = 0x0FFFFFFFu, ALWAYS = 1u << 30, FULL = 0xffffffffu;
   __shared__ TileQueue queues[TL_WARPS];
   TileQueue& q = queues[threadIdx.x >> 5];
@@ -316,36 +348,28 @@ __global__ void __launch_bounds__(TL_BLOCK) agg_tile_wide_kernel(const ColTable 
   const uint64_t pol = tl_policy_evict_first();
   const bool dec = ts.arg_is_dec != 0;
 
+  long long f[NF > 0 ? NF : 1][4]; unsigned fv[NF > 0 ? NF : 1];
+  tl_load_filters<NF>(cols, ts.frange, row_begin, gwarp * TL_ROWS + lane, n, pol, f, fv);
   for (long long tile = gwarp; tile < ntiles; tile += nwarps) {
-    const long long rel0 = tile * TL_ROWS + lane * 4, row0 = row_begin + rel0;
-    const int nrow = (int)(n - rel0 >= 4 ? 4 : (n - rel0 > 0 ? n - rel0 : 0));
-    long long f[NF > 0 ? NF : 1][4]; unsigned fv[NF > 0 ? NF : 1];
+    const long long rel0 = tile * TL_ROWS + lane, row0 = row_begin + rel0;
+    const unsigned alive = tl_pass<NF>(ts.frange, f, fv, tl_rows_in(rel0, n));       // filter first, as in agg_tile_dense_kernel
     long long k0[4], k1[4], a0[4], a1[4]; unsigned kv0, kv1 = 0xF, av0 = 0xF, av1 = 0xF;
-#pragma unroll
-    for (int c = 0; c < NF; c++) tl_load4(cols.col[ts.frange[c].col], ts.frange[c].phys, row0, nrow, true, pol, f[c], fv[c]);
-    tl_load4(cols.col[ts.key_col[0]], ts.key_phys[0], row0, nrow, true, pol, k0, kv0);
-    if (NK == 2) tl_load4(cols.col[ts.key_col[1]], ts.key_phys[1], row0, nrow, true, pol, k1, kv1);
+    tl_column<NF>(cols, ts.frange, f, fv, ts.key_col[0], ts.key_phys[0], row0, alive, true, pol, k0, kv0);
+    if (NK == 2) tl_column<NF>(cols, ts.frange, f, fv, ts.key_col[1], ts.key_phys[1], row0, alive, true, pol, k1, kv1);
     else { k1[0] = k1[1] = k1[2] = k1[3] = 0; }
     a0[0] = a0[1] = a0[2] = a0[3] = 0; a1[0] = a1[1] = a1[2] = a1[3] = 0;
     if (dec) {
-      tl_load4_dec(cols.col[ts.arg_col[0]], row0, nrow, pol, a0, a1, av0); av1 = av0;
+      tl_load_dec(cols.col[ts.arg_col[0]], row0, alive, pol, a0, a1, av0); av1 = av0;
       if (ts.dec_mul != 1) {                                         // TryCast to a larger scale (cannot overflow: the precision grows at least as much)
 #pragma unroll
         for (int j = 0; j < 4; j++) { const i128_t v = mk128((uint64_t)a0[j], (uint64_t)a1[j]) * (i128_t)ts.dec_mul; a0[j] = (long long)lo64(v); a1[j] = (long long)hi64(v); }
       }
     }
     else {
-      if (ts.nargs > 0) tl_load4(cols.col[ts.arg_col[0]], ts.arg_phys[0], row0, nrow, ts.arg_values[0] != 0, pol, a0, av0);
-      if (ts.nargs > 1) tl_load4(cols.col[ts.arg_col[1]], ts.arg_phys[1], row0, nrow, ts.arg_values[1] != 0, pol, a1, av1);
+      if (ts.nargs > 0) tl_column<NF>(cols, ts.frange, f, fv, ts.arg_col[0], ts.arg_phys[0], row0, alive, ts.arg_values[0] != 0, pol, a0, av0);
+      if (ts.nargs > 1) tl_column<NF>(cols, ts.frange, f, fv, ts.arg_col[1], ts.arg_phys[1], row0, alive, ts.arg_values[1] != 0, pol, a1, av1);
     }
-    unsigned alive = (1u << nrow) - 1u;
-#pragma unroll
-    for (int c = 0; c < NF; c++) {
-      unsigned pass = 0;
-#pragma unroll
-      for (int j = 0; j < 4; j++) pass |= (unsigned)((unsigned long long)(f[c][j] - ts.frange[c].lo) <= ts.frange[c].span) << j;
-      alive &= pass & fv[c];
-    }
+    tl_load_filters<NF>(cols, ts.frange, row_begin, rel0 + nwarps * TL_ROWS, n, pol, f, fv);   // the next tile's, in flight from here on
     const unsigned knull = (~kv0 | (NK == 2 ? ~kv1 : 0u)) & 0xFu;
     int total = 0; unsigned fb = 0;
 #pragma unroll
@@ -387,7 +411,7 @@ __global__ void __launch_bounds__(TL_BLOCK) agg_tile_wide_kernel(const ColTable 
           uint64_t kw[2] = {(kn & 1u) ? 0ULL : (uint64_t)k0[j], (NK == 2 && !(kn & 2u)) ? (uint64_t)k1[j] : 0ULL};
           unsigned fl = 0;
           const uint64_t si = agg_find_or_insert(lay, tab, kw, kn, agg_hash2(kw[0], kw[1], kn), &fl, &inserted);
-          if (si == AGG_NO_SLOT) { const unsigned long long at = atomicAdd(tab.counters + 1, 1ULL); tab.deferred[at] = (uint32_t)(rel0 + j); }
+          if (si == AGG_NO_SLOT) { const unsigned long long at = atomicAdd(tab.counters + 1, 1ULL); tab.deferred[at] = (uint32_t)(rel0 + 32 * j); }
           else tw_slot_update(lay, ts, tab.keys + si * (uint64_t)lay.kstride, tab.accs + si * (uint64_t)lay.astride, fl,
                               dec ? (unsigned long long)a0[j] : tw_convert(a0[j], ts.arg_cvt[0]), dec ? (unsigned long long)a1[j] : tw_convert(a1[j], ts.arg_cvt[1]),
                               (av0 >> j) & 1u, (av1 >> j) & 1u);
@@ -401,8 +425,8 @@ __global__ void __launch_bounds__(TL_BLOCK) agg_tile_wide_kernel(const ColTable 
 
 int launch_agg_tile_wide(const ColTable& cols, const TileAggSpec& ts, const AggLayout& lay, const AggTable& tab, int64_t row_begin, int64_t n, cudaStream_t s) {
   if (n <= 0 || ts.filt_never) return 0;
-  const int g = tile_grid((n + TL_ROWS - 1) / TL_ROWS, 4);
-#define B200Q_TW(NK, NF, G_, FL) agg_tile_wide_kernel<NK, NF, G_, FL><<<g, TL_BLOCK, 0, s>>>(cols, ts, lay, tab, row_begin, n)
+  const int64_t units = ((n + TL_ROWS - 1) / TL_ROWS + TL_WARPS - 1) / TL_WARPS;
+#define B200Q_TW(NK, NF, G_, FL) do { auto k_ = agg_tile_wide_kernel<NK, NF, G_, FL>; k_<<<tile_grid(k_, units), TL_BLOCK, 0, s>>>(cols, ts, lay, tab, row_begin, n); } while (0)
 #define B200Q_TW_FL(NK, NF, G_) do { if (ts.flavour == TF_ADD_U64) B200Q_TW(NK, NF, G_, TF_ADD_U64); else if (ts.flavour == TF_ADD_F64) B200Q_TW(NK, NF, G_, TF_ADD_F64); else B200Q_TW(NK, NF, G_, TF_MIN_S64); } while (0)
 #define B200Q_TW_G(NK, NF) do { if (ts.G == 2) B200Q_TW_FL(NK, NF, 2); else if (ts.G == 4) B200Q_TW_FL(NK, NF, 4); else B200Q_TW_FL(NK, NF, 8); } while (0)
 #define B200Q_TW_NF(NK) do { if (ts.nfcol == 0) B200Q_TW_G(NK, 0); else if (ts.nfcol == 1) B200Q_TW_G(NK, 1); else B200Q_TW_G(NK, 2); } while (0)
@@ -420,7 +444,7 @@ __global__ void __launch_bounds__(256) tile_wide_fill_kernel(unsigned long long*
 }
 int launch_tile_wide_init(const TileAggSpec& ts, cudaStream_t s) {
   const unsigned long long nwords = ts.dense_cap * (unsigned long long)ts.G;
-  tile_wide_fill_kernel<<<tile_grid((int64_t)((nwords + 1023) / 1024), 8), 256, 0, s>>>(ts.dense_tab, nwords, ts.flavour == TF_MIN_S64 ? 0x7FFFFFFFFFFFFFFFULL : 0ULL);
+  tile_wide_fill_kernel<<<tile_grid(tile_wide_fill_kernel, (int64_t)((nwords + 8191) / 8192)), 256, 0, s>>>(ts.dense_tab, nwords, ts.flavour == TF_MIN_S64 ? 0x7FFFFFFFFFFFFFFFULL : 0ULL);
   return 1;
 }
 __device__ __forceinline__ bool tw_present(const TileAggSpec& ts, const unsigned long long* e) {
@@ -434,7 +458,7 @@ __global__ void __launch_bounds__(256) tile_wide_count_kernel(const TileAggSpec 
   if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
 }
 int launch_tile_wide_count(const TileAggSpec& ts, unsigned long long* d_out, cudaStream_t s) {
-  tile_wide_count_kernel<<<tile_grid(((int64_t)ts.dense_cap + 2047) / 2048, 8), 256, 0, s>>>(ts, d_out);
+  tile_wide_count_kernel<<<tile_grid(tile_wide_count_kernel, ((int64_t)ts.dense_cap + 16383) / 16384), 256, 0, s>>>(ts, d_out);
   return 1;
 }
 // decimal128 SUM pieces {low 32 bits, middle 32 bits, high 64 bits} accumulated with 64-bit adds: move the carries up
@@ -448,7 +472,7 @@ __global__ void __launch_bounds__(256) tile_wide_normalise_kernel(const TileAggS
 }
 int launch_tile_wide_normalise(const TileAggSpec& ts, cudaStream_t s) {
   if (ts.dec_word == 0xFF) return 0;
-  tile_wide_normalise_kernel<<<tile_grid(((int64_t)ts.dense_cap + 2047) / 2048, 8), 256, 0, s>>>(ts);
+  tile_wide_normalise_kernel<<<tile_grid(tile_wide_normalise_kernel, ((int64_t)ts.dense_cap + 16383) / 16384), 256, 0, s>>>(ts);
   return 1;
 }
 __global__ void __launch_bounds__(256) tile_wide_emit_kernel(const TileAggSpec ts, const AggLayout lay, const EmitTable emit, unsigned long long* out_count) {
@@ -496,7 +520,7 @@ __global__ void __launch_bounds__(256) tile_wide_emit_kernel(const TileAggSpec t
   }
 }
 int launch_tile_wide_emit(const TileAggSpec& ts, const AggLayout& lay, const EmitTable& emit, unsigned long long* d_out_count, cudaStream_t s) {
-  tile_wide_emit_kernel<<<tile_grid(((int64_t)ts.dense_cap + 2047) / 2048, 8), 256, 0, s>>>(ts, lay, emit, d_out_count);
+  tile_wide_emit_kernel<<<tile_grid(tile_wide_emit_kernel, ((int64_t)ts.dense_cap + 16383) / 16384), 256, 0, s>>>(ts, lay, emit, d_out_count);
   return 1;
 }
 

@@ -116,6 +116,19 @@ m2 = PL.AggExec(PL.HashAgg, [E.GroupingExpr("k1", E.Column("k1")), E.GroupingExp
                 [E.AggExpr("s", E.PARTIAL, PL.create_agg(E.AGG_SUM, [E.Column("v")], s2, T.int64))], True, PL.FilterExec(preds, PL.MemoryExec(s2)))
 run("M2 q1-shaped fused filter->agg (2 keys)", m2.plan_bytes(), [f, k1, k2, v], 32.0, native.default_conf(agg_initial_groups=1 << 20))
 run("M2 q1-shaped", m2.plan_bytes(), [f, k1, k2, v], 32.0, native.default_conf(agg_initial_groups=1 << 20), reps=1, steady=True)
+# M2 selectivity sweep: the tile kernel reads k1, k2 and v only for the rows that pass, so s = 1.0 guards against that costing
+# more than reading every column at once
+m2s = lambda sch, lo, hi: PL.AggExec(PL.HashAgg, [E.GroupingExpr("k1", E.Column("k1")), E.GroupingExpr("k2", E.Column("k2"))],
+                                     [E.AggExpr("s", E.PARTIAL, PL.create_agg(E.AGG_SUM, [E.Column("v")], sch, T.int64))], True,
+                                     PL.FilterExec([E.BinaryExpr(E.Column("f"), "GtEq", E.Literal(lo, T.int64)), E.BinaryExpr(E.Column("f"), "LtEq", E.Literal(hi, T.int64))], PL.MemoryExec(sch)))
+for sel in (0.01, 0.2, 0.5, 1.0):
+    run("M2 selectivity s=%.2f" % sel, m2s(s2, 0, int(1000 * sel) - 1).plan_bytes(), [f, k1, k2, v], 32.0, native.default_conf(agg_initial_groups=1 << 20))
+# M2 with an int32 key and a nullable value (10 % NULL)  (28.125 B/row)
+k1_32 = k1.to(torch.int32)
+vbits = torch.full(((rows + 7) // 8,), 0xFF, dtype=torch.uint8, device=dev); vbits[::10] = 0
+s2t = T.Schema([T.Field("f", T.int64, False), T.Field("k1", T.int32, False), T.Field("k2", T.int64, False), T.Field("v", T.int64, True)])
+run("M2 int32 key, nullable v", m2s(s2t, 200, 399).plan_bytes(), [f, k1_32, k2, v], 28.125, native.default_conf(agg_initial_groups=1 << 20), valid=[None, None, None, vbits])
+del k1_32, vbits
 # M3: ShuffleWriterExec 200-way hash partition + batch_serde encode (BASELINE configs[3] map side): 32 B/row read + 32 B/row of byte planes written
 m3 = PL.ShuffleWriterExec(PL.MemoryExec(s2), ("hash", [E.Column("k1")], 200), "", "")
 run("M3 shuffle write 200-way (4 int64 columns, hash on k1)", m3.plan_bytes(), [f, k1, k2, v], 64.0, native.default_conf(shuffle_output_on_device=1), reps=2)

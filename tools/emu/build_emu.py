@@ -19,6 +19,8 @@ def translate(m):
     outs = OPERAND.findall(parts[1]) if len(parts) > 1 else []
     ins = OPERAND.findall(parts[2]) if len(parts) > 2 else []
     op = ptx.split()[0]
+    if ptx.startswith("{") and re.search(r"@\w+ ld\.global\.nc", ptx):          # `setp` + predicated load: (pointer, predicate, policy) -> "+" outputs
+        return f"if ({ins[1]}) {{ " + " ".join(f"{o} = ({ins[0]})[{i}];" for i, o in enumerate(outs)) + " }"
     if "mbarrier" in ptx or "cp.async.bulk" in ptx or op.startswith("fence."): return ";"      # TMA staging: never reached on the emulated device (compiled out)
     if op == "ld.relaxed.gpu.global.u64": return f"{outs[0]} = emu_ld64({ins[0]});"
     if op == "ld.relaxed.gpu.global.v2.u64": return f"{outs[0]} = emu_ld64({ins[0]}); {outs[1]} = emu_ld64({ins[0]} + 1);"

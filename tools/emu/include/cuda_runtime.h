@@ -133,6 +133,7 @@ inline cudaError_t cudaGetDeviceCount(int* n) { *n = 1; return cudaSuccess; }
 inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
 inline cudaError_t cudaDeviceGetAttribute(int* v, int, int) { *v = 1; return cudaSuccess; }   // one "SM": small grids
+template <class F> inline cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int* v, F, int, size_t) { *v = 1; return cudaSuccess; }
 inline cudaError_t cudaDeviceGetDefaultMemPool(cudaMemPool_t* p, int) { *p = nullptr; return cudaSuccess; }
 inline cudaError_t cudaMemPoolSetAttribute(cudaMemPool_t, int, void*) { return cudaSuccess; }
 inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) { *s = (cudaStream_t)malloc(8); return cudaSuccess; }
