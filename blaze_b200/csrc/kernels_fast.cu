@@ -837,8 +837,9 @@ __global__ void __launch_bounds__(256) agg_emit_dense_kernel(const FastSpec fs, 
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   const uint64_t rounds = (fs.dense_cap + stride - 1) / stride;
   for (uint64_t it = 0; it < rounds; it++) {
-    const uint64_t i = it * stride + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-    const unsigned long long* e = fs.dense_tab + i * fs.dense_stride;
+    const uint64_t i = it * stride + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;   // key order: (key0 - dense_base) * dense_r1 + (key1 - dense_base1)
+    const uint64_t pe = fs.nkeys == 2 && fs.dense_key0_minor ? dense_entry2(fs, i / fs.dense_r1, i % fs.dense_r1) : i;
+    const unsigned long long* e = fs.dense_tab + pe * fs.dense_stride;
     const bool occ = i < fs.dense_cap && e[fs.dense_presence_word] != 0;
     const unsigned m = __ballot_sync(0xffffffffu, occ);
     if (!m) continue;

@@ -23,13 +23,15 @@ struct FastSpec {
   FilterInterval frange[2];
   long long dense_base;                                   // DENSE: entry index = key0 - dense_base                      (one key)
   unsigned long long dense_cap;                           // entries of dense_stride words
-  long long dense_base1;                                  //        entry index = (key0 - dense_base) * dense_r1 + (key1 - dense_base1)   (two keys)
+  long long dense_base1;                                  //        entry index = (key0 - dense_base) * dense_r1 + (key1 - dense_base1)   (two keys),
+                                                          //        or (key1 - dense_base1) * dense_cap0 + (key0 - dense_base) with dense_key0_minor
   unsigned long long dense_r1, dense_cap0;                // key1 - dense_base1 < dense_r1, key0 - dense_base < dense_cap0; dense_cap = dense_cap0 * dense_r1
   unsigned long long* dense_tab;
   int8_t dense_stride;                                    // 2 or 4 words per entry (= lanes that update one entry in one instruction)
   int8_t dense_word_src[4];                               // per entry word: -1 row counter (+1), -2 padding (+0), j accumulator j, 2+j valid arguments of accumulator j
   uint8_t dense_presence_word;                            // word that is non-zero iff the entry holds a group
-  uint8_t _pad1[2];
+  uint8_t dense_key0_minor;                               // two keys: key0 varies fastest in the entry index (set when key1 has the shorter span)
+  uint8_t _pad1;
   unsigned long long* sink;                               // FAST_SINK_WARPS x 4 words: per-warp scratch sector for no-op REDs
 };
 constexpr int FAST_SINK_WARPS = 4096;
@@ -37,13 +39,17 @@ constexpr int FAST_SINK_WARPS = 4096;
 // per emit column: which dense word holds the value and which (count) word validates it
 struct DenseEmitMap { uint8_t word[EMIT_MAX_COLS]; uint8_t valid_word[EMIT_MAX_COLS]; };
 
+// entry of the two-key offsets d0 < dense_cap0, d1 < dense_r1
+__device__ __forceinline__ unsigned long long dense_entry2(const FastSpec& fs, unsigned long long d0, unsigned long long d1) {
+  return fs.dense_key0_minor ? d1 * fs.dense_cap0 + d0 : d0 * fs.dense_r1 + d1;
+}
 // dense entry index of a row; false: outside the dense range (the row goes to a hashed slot)
 template <int NK>
 __device__ __forceinline__ bool dense_index_of(const FastSpec& fs, long long k0, long long k1, unsigned long long& idx) {
   const unsigned long long d0 = (unsigned long long)(k0 - fs.dense_base);
   if (NK == 1) { idx = d0; return d0 < fs.dense_cap; }
   const unsigned long long d1 = (unsigned long long)(k1 - fs.dense_base1);
-  idx = d0 * fs.dense_r1 + d1;
+  idx = dense_entry2(fs, d0, d1);
   return d0 < fs.dense_cap0 && d1 < fs.dense_r1;
 }
 
