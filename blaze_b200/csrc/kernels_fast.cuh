@@ -67,6 +67,13 @@ __device__ __forceinline__ bool dense_index_of(const FastSpec& fs, long long k0,
 // NULL / out-of-range keys fall back to the hashed table with the generic accumulator updates of AggLayout.
 // ---------------------------------------------------------------------------------------------------
 enum TileFlavour : uint8_t { TF_ADD_U64 = 0, TF_ADD_F64 = 1, TF_MIN_S64 = 2 };
+// identity of a flavour's RED: the fill of every dense word and the value a gated-off lane adds.  f64 words start at -0.0,
+// the identity of IEEE addition (-0.0 + x == x for every x): a group whose values are all -0.0 sums to -0.0, as the
+// reference's store-the-first-value-then-add does, where +0.0 would turn it into +0.0.  Marks and counts are therefore
+// tested as doubles under TF_ADD_F64 (tw_marked), not as integers
+__host__ __device__ constexpr unsigned long long tile_identity(int flavour) {
+  return flavour == TF_MIN_S64 ? 0x7FFFFFFFFFFFFFFFULL : flavour == TF_ADD_F64 ? 0x8000000000000000ULL : 0ULL;
+}
 enum TileArgCvt : uint8_t { TC_NONE = 0, TC_I2F = 1 /* integer -> f64 bits */, TC_ORDER = 2 /* f64 bits -> totalOrder key */ };
 enum TileRecon : uint8_t { TR_COPY = 0 /* slot word = dense word */, TR_NOT = 1 /* ~dense word (a maximum kept as the minimum of the complement) */,
                            TR_F2I = 2 /* count kept as f64 */, TR_DEC3 = 3 /* three carry-free pieces -> {lo, hi} */ };

@@ -289,7 +289,7 @@ template <int FLAV> __device__ __forceinline__ void tw_red(unsigned long long* p
   else if (FLAV == TF_ADD_F64) red_add_f64(p, as_f64(v));
   else red_min_s64(p, (long long)v);
 }
-template <int FLAV> __device__ __forceinline__ unsigned long long tw_noop() { return FLAV == TF_MIN_S64 ? 0x7FFFFFFFFFFFFFFFULL : 0ULL; }
+template <int FLAV> __device__ __forceinline__ unsigned long long tw_noop() { return tile_identity(FLAV); }
 
 // rows r0 + 32 j of one decimal128 column (bit j of `ld`): low and high words, one 128-bit load per row when the column is
 // 16-byte aligned (an Arrow slice of an 8-byte aligned buffer may not be: two 64-bit loads)
@@ -444,12 +444,15 @@ __global__ void __launch_bounds__(256) tile_wide_fill_kernel(unsigned long long*
 }
 int launch_tile_wide_init(const TileAggSpec& ts, cudaStream_t s) {
   const unsigned long long nwords = ts.dense_cap * (unsigned long long)ts.G;
-  tile_wide_fill_kernel<<<tile_grid(tile_wide_fill_kernel, (int64_t)((nwords + 8191) / 8192)), 256, 0, s>>>(ts.dense_tab, nwords, ts.flavour == TF_MIN_S64 ? 0x7FFFFFFFFFFFFFFFULL : 0ULL);
+  tile_wide_fill_kernel<<<tile_grid(tile_wide_fill_kernel, (int64_t)((nwords + 8191) / 8192)), 256, 0, s>>>(ts.dense_tab, nwords, tile_identity(ts.flavour));
   return 1;
 }
-__device__ __forceinline__ bool tw_present(const TileAggSpec& ts, const unsigned long long* e) {
-  return ts.flavour == TF_MIN_S64 ? e[ts.presence_word] == 0 : e[ts.presence_word] != 0;
+// a presence / valid-argument word has seen a row: MIN(0) under TF_MIN_S64, a non-zero count otherwise (an f64 count
+// starts at -0.0, whose bits are not 0)
+__device__ __forceinline__ bool tw_marked(const TileAggSpec& ts, unsigned long long w) {
+  return ts.flavour == TF_MIN_S64 ? w == 0 : ts.flavour == TF_ADD_F64 ? as_f64(w) != 0.0 : w != 0;
 }
+__device__ __forceinline__ bool tw_present(const TileAggSpec& ts, const unsigned long long* e) { return tw_marked(ts, e[ts.presence_word]); }
 __global__ void __launch_bounds__(256) tile_wide_count_kernel(const TileAggSpec ts, unsigned long long* out) {
   unsigned long long c = 0;
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < ts.dense_cap; i += (uint64_t)gridDim.x * blockDim.x) c += tw_present(ts, ts.dense_tab + i * ts.G);
@@ -479,7 +482,6 @@ __global__ void __launch_bounds__(256) tile_wide_emit_kernel(const TileAggSpec t
   const unsigned lane = threadIdx.x & 31;
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   const uint64_t rounds = (ts.dense_cap + stride - 1) / stride;
-  const bool is_min = ts.flavour == TF_MIN_S64;
   for (uint64_t it = 0; it < rounds; it++) {
     const uint64_t i = it * stride + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
     const unsigned long long* e = ts.dense_tab + i * ts.G;
@@ -513,7 +515,7 @@ __global__ void __launch_bounds__(256) tile_wide_emit_kernel(const TileAggSpec t
         }
       }
       const uint8_t vw = ts.acc[a].valid_word;
-      const bool valid = vw == 0xFF ? true : (is_min ? e[vw] == 0 : e[vw] != 0);
+      const bool valid = vw == 0xFF ? true : tw_marked(ts, e[vw]);
       if (op.vbit != 0xFF && valid) flags |= 1u << op.vbit;
     }
     emit_row_columns(emit, at, ke, slot, flags);

@@ -559,7 +559,7 @@ class AggStage : public Stage {
         AccKind kind; int nwords = 1; uint64_t ilo = 0, ihi = 0;
         if (a.fn == AGG_SUM || a.fn == AGG_AVG) {
           if (dt.is_decimal()) { kind = ACC_ADD_DEC; nwords = 2; }
-          else if (dt.id == T_FLOAT64) kind = ACC_ADD_F64;
+          else if (dt.id == T_FLOAT64) { kind = ACC_ADD_F64; ilo = 0x8000000000000000ULL; }   // -0.0: see tile_identity
           else if (dt.is_integer()) kind = ACC_ADD_I64;
           else throw PlanError(B200Q_ERR_UNSUPPORTED, "sum/avg accumulating at " + dt.str() + " is not on the hot path");
         } else {
@@ -818,7 +818,7 @@ class AggStage : public Stage {
     if ((int)any_f64 + (int)any_min + (int)any_int > 1) return;
     ts.flavour = any_f64 ? TF_ADD_F64 : any_min ? TF_MIN_S64 : TF_ADD_U64;
     const unsigned long long ONE = ts.flavour == TF_ADD_F64 ? 0x3FF0000000000000ULL : ts.flavour == TF_MIN_S64 ? 0ULL : 1ULL;
-    const unsigned long long NOOP = ts.flavour == TF_MIN_S64 ? 0x7FFFFFFFFFFFFFFFULL : 0ULL;
+    const unsigned long long NOOP = tile_identity(ts.flavour);
     // argument columns
     struct ArgInfo { int col_index; int cvt; bool nullable; bool values; };
     std::vector<ArgInfo> args; std::vector<ExprP> arg_cols;

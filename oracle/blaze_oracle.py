@@ -117,10 +117,11 @@ def col_from_arrow(arr) -> Col:
     n = len(arr)
     valid = np.ones(n, bool) if arr.null_count == 0 else np.array(arr.is_valid().to_pylist(), bool)
     if dt.id == T.DECIMAL128:
+        # the unscaled 128-bit words themselves: a Decimal through the default 28-digit context would round them
+        words = np.frombuffer(arr.buffers()[1], dtype="<u8", count=2 * (arr.offset + n))[2 * arr.offset:] if n else []
         vals = np.empty(n, object)
-        s = dt.scale
-        for i, v in enumerate(arr.to_pylist()):
-            vals[i] = 0 if v is None else int(v.scaleb(s).to_integral_value())
+        for i in range(n):
+            vals[i] = wrap_i128(int(words[2 * i]) | int(words[2 * i + 1]) << 64) if valid[i] else 0
     elif dt.id == T.BINARY:
         vals = np.empty(n, object)
         for i, v in enumerate(arr.to_pylist()):
