@@ -221,6 +221,54 @@ static void build_pipeline(b200q_op* op) {
       }
       op->stages.push_back(make_sort_stage(op->cx, stage_in, *n));
       stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in);
+    } else if (n->kind == N_WINDOW) {
+      // a WindowExec without a limit directly on one with a limit runs as ONE window: the parent's expressions, the child's
+      // limit, output_window_cols = true, over the child's input (window_exec.rs:166-185)
+      PlanNode combined;
+      const PlanNode* w = n;
+      if (n->window_has_limit && i + 1 < chain.size() && chain[i + 1]->kind == N_WINDOW && !chain[i + 1]->window_has_limit) {
+        if (n->output_window_cols) throw PlanError(B200Q_ERR_UNSUPPORTED, "WindowExec over a group-limited WindowExec that outputs its window column");
+        // the combined window outputs its window columns whatever the parent declares: a parent without them would disagree with it
+        if (!chain[i + 1]->output_window_cols) throw PlanError(B200Q_ERR_UNSUPPORTED, "WindowExec with output_window_cols = false over a group-limited WindowExec");
+        combined = *chain[i + 1]; combined.window_has_limit = true; combined.window_limit = n->window_limit; combined.output_window_cols = true;
+        if (combined.window_exprs.size() != 1) throw PlanError(B200Q_ERR_INVALID_PLAN, "WindowExec: a group limit needs exactly one window expression, got " + std::to_string(combined.window_exprs.size()));
+        if (!combined.window_exprs[0].is_rank) throw PlanError(B200Q_ERR_UNSUPPORTED, "WindowExec: a group limit over an aggregate window column is not on the GPU path (rank-like functions are)");
+        w = &combined; i++; last = chain[i];
+      }
+      // keys and arguments that are not input columns are computed by a FilterProjectStage below, as trailing columns
+      const size_t n_fwd = w->input->schema.fields.size();
+      std::vector<ExprP> extra;
+      SchemaDef win_in = w->input->schema;
+      auto col_of = [&](ExprP e) {
+        while ((e->kind == E_TRY_CAST || e->kind == E_CAST) && e->children[0]->type == e->type) e = e->children[0];   // create_agg's TryCast to the type it has
+        if (e->kind == E_COLUMN) return e->col_index;
+        extra.push_back(e);
+        win_in.fields.push_back(FieldDef{"#window_arg" + std::to_string(extra.size() - 1), e->type, e->nullable});
+        return (int)(n_fwd + extra.size() - 1);
+      };
+      WindowCols wc; wc.n_fwd = n_fwd;
+      for (auto& e : w->window_partition) wc.partition_cols.push_back(col_of(e));
+      for (auto& se : w->window_order) wc.order_cols.push_back(col_of(se.expr));
+      for (auto& we : w->window_exprs) { std::vector<int> v; if (!we.is_rank) for (auto& a : we.agg.args) v.push_back(col_of(a)); wc.agg_args.push_back(v); }
+      if (pending_tail || !extra.empty()) {
+        std::vector<ExprP> outs = cur_cols;
+        for (auto& e : extra) outs.push_back(substitute(e, cur_cols));
+        op->stages.push_back(make_filter_project_stage(op->cx, stage_in, filters, outs, win_in));
+        filters.clear(); pending_tail = false;
+      }
+      op->stages.push_back(make_window_stage(op->cx, win_in, *w, wc));
+      stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in);
+      if (w->window_has_limit) {
+        // WindowGroupLimit: keep the rows whose window column is <= (int32)k (window_exec.rs:227-235); the window column is dropped
+        // unless output_window_cols.  A pending filter, fused into whatever runs next.
+        auto col = cur_cols[n_fwd];
+        auto lit = std::make_shared<Expr>(); lit->kind = E_LITERAL; lit->type.id = T_INT32; lit->nullable = false;
+        lit->lit_lo = (uint64_t)(int64_t)(int32_t)w->window_limit;
+        auto le = std::make_shared<Expr>(); le->kind = E_BINARY; le->op = OP_LE; le->type.id = T_BOOL; le->nullable = col->nullable; le->children = {col, lit};
+        filters.push_back(le);
+        if (!w->output_window_cols) cur_cols.resize(n_fwd);
+        pending_tail = true;
+      }
     } else if (n->kind == N_JOIN_BUILD || n->kind == N_JOIN) {
       if (pending_tail) {                               // Filter / Project chain below the join side: its own fused stage
         op->stages.push_back(make_filter_project_stage(op->cx, stage_in, filters, cur_cols, n->input->schema));

@@ -7,6 +7,14 @@
 
 namespace b200q {
 
+// AVG results from (sum, count != 0): f64 division, and i128::checked_div_euclid for decimals (avg.rs:158-165)
+__device__ __forceinline__ double avg_f64_final(double sum, long long cnt) { return sum / __ll2double_rn(cnt); }
+__device__ __forceinline__ i128_t avg_dec_final(i128_t sum, long long cnt) {
+  i128_t q = sum / cnt; const i128_t r = sum % cnt;
+  if (r < 0) q += cnt > 0 ? -1 : 1;
+  return q;
+}
+
 __device__ __forceinline__ void emit_store(const EmitCol& c, unsigned long long at, uint64_t lo, uint64_t hi, bool valid) {
   if (c.valid_bytes) c.valid_bytes[at] = valid ? 1 : 0;
   switch (c.phys) {
@@ -41,18 +49,13 @@ __device__ __forceinline__ void emit_row_columns(const EmitTable& emit, unsigned
           const long long cnt = (long long)slot[ec.word2];
           const bool valid = (ec.vbit == 0xFF ? true : ((flags >> ec.vbit) & 1)) && cnt != 0;
           const double sum = ec.sum_is_f64 ? as_f64(slot[ec.word]) : __ll2double_rn((long long)slot[ec.word]);
-          emit_store(ec, at, valid ? f64_bits(sum / __ll2double_rn(cnt)) : 0, 0, valid);
+          emit_store(ec, at, valid ? f64_bits(avg_f64_final(sum, cnt)) : 0, 0, valid);
           break;
         }
         default: {   // EMIT_AVG_DEC: i128::checked_div_euclid(sum, count) (avg.rs:158-165)
           const long long cnt = (long long)slot[ec.word2];
           const bool valid = (ec.vbit == 0xFF ? true : ((flags >> ec.vbit) & 1)) && cnt != 0;
-          i128_t q = 0;
-          if (valid) {
-            const i128_t sum = mk128(slot[ec.word], slot[ec.word + 1]);
-            q = sum / cnt; const i128_t r = sum % cnt;
-            if (r < 0) q += cnt > 0 ? -1 : 1;
-          }
+          const i128_t q = valid ? avg_dec_final(mk128(slot[ec.word], slot[ec.word + 1]), cnt) : 0;
           emit_store(ec, at, lo64(q), hi64(q), valid);
           break;
         }

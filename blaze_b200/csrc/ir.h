@@ -102,7 +102,7 @@ struct AggDef {
   }
 };
 
-enum NodeKind : uint8_t { N_LEAF, N_FILTER, N_PROJECT, N_AGG, N_SHUFFLE_WRITER, N_JOIN_BUILD, N_JOIN, N_SORT, N_EXPAND };
+enum NodeKind : uint8_t { N_LEAF, N_FILTER, N_PROJECT, N_AGG, N_SHUFFLE_WRITER, N_JOIN_BUILD, N_JOIN, N_SORT, N_EXPAND, N_WINDOW };
 enum ShuffleKind : uint8_t { SHUFFLE_SINGLE = 0, SHUFFLE_HASH = 1, SHUFFLE_ROUND_ROBIN = 2, SHUFFLE_RANGE = 3 };   // PhysicalRepartition oneof (auron.proto:629-655)
 
 struct PlanNode {
@@ -153,8 +153,27 @@ struct PlanNode {
   // N_EXPAND (ExpandExecNode, auron.proto:714-722): one expression per schema field in every projection, resolved against
   // the input schema, of exactly the field's type (expressions beyond the field count are dropped at decode)
   std::vector<std::vector<ExprP>> expand_projections;
+  // N_WINDOW (WindowExecNode / WindowExprNode, auron.proto:537-562): expressions resolved against the input schema.  Output =
+  // input columns ++ (output_window_cols ? one column per window expression : nothing)
+  struct WindowExprDef {
+    FieldDef field;
+    bool is_rank = true;
+    int rank_fn = 0;                       // WindowFunction: 0 ROW_NUMBER, 1 RANK, 2 DENSE_RANK
+    AggDef agg;                            // is_rank false: args after create_agg rewriting (as AggExec), mode Partial
+  };
+  std::vector<WindowExprDef> window_exprs;
+  std::vector<ExprP> window_partition;
+  std::vector<SortExprDef> window_order;
+  bool window_has_limit = false;
+  uint32_t window_limit = 0;
+  bool output_window_cols = false;
 };
 using PlanP = std::shared_ptr<PlanNode>;
+
+// WindowExec limits, refused at decode (UNSUPPORTED)
+constexpr int WINDOW_MAX_EXPRS = 8;        // window expressions of one node
+constexpr int WINDOW_MAX_KEYS = 16;        // partition + order keys
+constexpr int WINDOW_MAX_COUNT_ARGS = 4;   // nullable COUNT arguments
 
 // plan_decode.cc
 PlanP decode_plan(const uint8_t* bytes, size_t n, int plan_kind);

@@ -110,22 +110,25 @@ DType parse_arrow_type(Reader r) {
   return d;
 }
 
-SchemaDef parse_schema(Reader r) {            // Schema{columns=1}; Field{name=1,arrow_type=2,nullable=3}
+FieldDef parse_field(Reader c) {               // Field{name=1,arrow_type=2,nullable=3}
+  FieldDef fd; fd.nullable = false; bool have_t = false;
+  while (!c.done()) {
+    int w; uint32_t g = c.tag(w);
+    if (g == 1) fd.name = c.str();
+    else if (g == 2) { fd.type = parse_arrow_type(c.bytes()); have_t = true; }
+    else if (g == 3) fd.nullable = c.varint() != 0;
+    else c.skip(w);
+  }
+  if (!have_t) bad("Field without arrow_type");
+  return fd;
+}
+
+SchemaDef parse_schema(Reader r) {            // Schema{columns=1}
   SchemaDef s;
   while (!r.done()) {
     int wt; uint32_t f = r.tag(wt);
-    if (f == 1) {
-      Reader c = r.bytes(); FieldDef fd; fd.nullable = false; bool have_t = false;
-      while (!c.done()) {
-        int w; uint32_t g = c.tag(w);
-        if (g == 1) fd.name = c.str();
-        else if (g == 2) { fd.type = parse_arrow_type(c.bytes()); have_t = true; }
-        else if (g == 3) fd.nullable = c.varint() != 0;
-        else c.skip(w);
-      }
-      if (!have_t) bad("Field without arrow_type");
-      s.fields.push_back(fd);
-    } else r.skip(wt);
+    if (f == 1) s.fields.push_back(parse_field(r.bytes()));
+    else r.skip(wt);
   }
   return s;
 }
@@ -644,6 +647,105 @@ PlanP parse_expand(Reader r) {
   return n;
 }
 
+// WindowExecNode{input=1, window_expr=2, partition_spec=3, order_spec=4, group_limit=5{k=1}, output_window_cols=6},
+// WindowExprNode{field=1, return_type=1000, func_type=2, window_func=3, agg_func=4, children=5} (from_proto.rs:535-668),
+// validated like WindowContext::try_new and create_agg (agg/agg.rs:171-205)
+PlanP parse_window(Reader r) {
+  auto n = std::make_shared<PlanNode>(); n->kind = N_WINDOW;
+  std::vector<Reader> wexprs, parts, orders;
+  while (!r.done()) {
+    int wt; uint32_t f = r.tag(wt);
+    switch (f) {
+      case 1: n->input = parse_plan(r.bytes()); break;
+      case 2: wexprs.push_back(r.bytes()); break;
+      case 3: parts.push_back(r.bytes()); break;
+      case 4: orders.push_back(r.bytes()); break;
+      case 5: { Reader gl = r.bytes(); n->window_has_limit = true; while (!gl.done()) { int w2; uint32_t g = gl.tag(w2); if (g == 1) n->window_limit = (uint32_t)gl.varint(); else gl.skip(w2); } break; }
+      case 6: n->output_window_cols = r.varint() != 0; break;
+      default: r.skip(wt);
+    }
+  }
+  if (!n->input) bad("Missing required field in protobuf");
+  const SchemaDef& in = n->input->schema;
+  auto check_key = [](const ExprP& e, const char* what) {
+    if (e->type.is_varlen() || e->type.id == T_NULL) unsupported(std::string("WindowExec: ") + what + " key of type " + e->type.str() + " is not on the GPU path");
+  };
+  for (auto& p : parts) { n->window_partition.push_back(parse_expr(p, in)); check_key(n->window_partition.back(), "partition"); }
+  for (auto& o : orders) {
+    Reader er = o; bool found = false; PlanNode::SortExprDef d; d.asc = false; d.nulls_first = false;
+    while (!er.done()) {
+      int wt; uint32_t f = er.tag(wt);
+      if (f != 11) { er.skip(wt); continue; }
+      Reader sr = er.bytes(); found = true;
+      while (!sr.done()) { int w2; uint32_t g = sr.tag(w2); if (g == 1) d.expr = parse_expr(sr.bytes(), in); else if (g == 2) d.asc = sr.varint() != 0; else if (g == 3) d.nulls_first = sr.varint() != 0; else sr.skip(w2); }
+    }
+    if (!found) bad("physical_plan::from_proto() Unexpected expr: a window order_spec entry is not a PhysicalSortExprNode");
+    if (!d.expr) bad("physical_plan::from_proto() Unexpected sort expr: sort expression without an expression");
+    check_key(d.expr, "order");
+    n->window_order.push_back(d);
+  }
+  if (n->window_partition.size() + n->window_order.size() > (size_t)WINDOW_MAX_KEYS)
+    unsupported("WindowExec with more than " + std::to_string(WINDOW_MAX_KEYS) + " partition + order keys is not on the GPU path");
+  for (auto& wr : wexprs) {
+    Reader er = wr; PlanNode::WindowExprDef w; bool have_field = false, have_rt = false; DType rt; uint64_t func_type = 0, wfn = 0, afn = 0;
+    std::vector<ExprP> children;
+    while (!er.done()) {
+      int wt; uint32_t f = er.tag(wt);
+      if (f == 1) { w.field = parse_field(er.bytes()); have_field = true; }
+      else if (f == 1000) { rt = parse_arrow_type(er.bytes()); have_rt = true; }
+      else if (f == 2) func_type = er.varint(); else if (f == 3) wfn = er.varint(); else if (f == 4) afn = er.varint();
+      else if (f == 5) children.push_back(parse_expr(er.bytes(), in));
+      else er.skip(wt);
+    }
+    if (!have_field) bad("physical_plan::from_proto() Unexpected sort expr: window expression without a field");
+    if (!have_rt) bad("Missing required field in protobuf");
+    DType out;
+    if (func_type == 0) {
+      if (wfn > 2) bad("invalid WindowFunction");
+      w.is_rank = true; w.rank_fn = (int)wfn; out.id = T_INT32;
+    } else if (func_type == 1) {
+      static const char* names[] = {"MIN", "MAX", "SUM", "AVG", "COUNT", "COLLECT_LIST", "COLLECT_SET", "FIRST", "FIRST_IGNORES_NULL", "BLOOM_FILTER"};
+      if (afn > 4) {
+        if (afn <= 9 || (afn >= 1000 && afn <= 1002)) unsupported(std::string("window aggregate ") + (afn <= 9 ? names[afn] : afn == 1002 ? "UDAF" : "BRICKHOUSE") + " is not on the GPU path (MIN / MAX / SUM / AVG / COUNT are)");
+        bad("invalid AggFunction");
+      }
+      w.is_rank = false;
+      AggDef& a = w.agg; a.fn = (AggFn)afn; a.mode = MODE_PARTIAL; a.field_name = w.field.name;
+      if (a.fn == AGG_COUNT) {
+        a.data_type = i64_t();
+        for (auto& c : children) if (c->nullable) a.args.push_back(c);
+        if (a.args.size() > (size_t)WINDOW_MAX_COUNT_ARGS) unsupported("window COUNT of more than " + std::to_string(WINDOW_MAX_COUNT_ARGS) + " nullable arguments is not on the GPU path");
+      } else {
+        if (children.empty()) bad("aggregate without children");
+        const DType ct = children[0]->type;
+        if (a.fn == AGG_SUM || a.fn == AGG_AVG) {
+          if (ct.is_varlen()) unsupported(std::string("window ") + (a.fn == AGG_SUM ? "SUM" : "AVG") + " over a " + ct.str() + " column is not on the GPU path");
+          if (a.fn == AGG_SUM && !(rt.is_integer() || rt.id == T_FLOAT64 || rt.is_decimal())) unsupported("window SUM accumulating at " + rt.str() + " is not on the GPU path");
+          if (a.fn == AGG_AVG && !(rt.id == T_FLOAT64 || rt.is_decimal())) unsupported("window AVG returning " + rt.str() + " is not on the GPU path");
+          check_cast_supported(ct, rt, true);
+          a.data_type = rt;
+          a.args.push_back(wrap_try_cast(children[0], rt));
+        } else {
+          if (ct.id == T_BOOL || ct.is_varlen() || ct.id == T_NULL) unsupported(std::string("window ") + (a.fn == AGG_MIN ? "MIN" : "MAX") + " over " + ct.str() + " is not on the GPU path");
+          a.data_type = ct;
+          a.args.push_back(children[0]);
+        }
+      }
+      out = a.data_type;
+    } else bad("invalid WindowFunctionType");
+    if (out != w.field.type) unsupported("WindowExec: window column " + w.field.name + " is computed as " + out.str() + " but its field is " + w.field.type.str() + " (the cast is not on the GPU path)");
+    n->window_exprs.push_back(w);
+  }
+  if (n->window_exprs.size() > (size_t)WINDOW_MAX_EXPRS) unsupported("WindowExec with more than " + std::to_string(WINDOW_MAX_EXPRS) + " window expressions is not on the GPU path");
+  if (n->window_has_limit) {
+    if (n->window_exprs.size() != 1) bad("WindowExec: a group limit needs exactly one window expression, got " + std::to_string(n->window_exprs.size()));   // window_exec.rs:228
+    if (!n->window_exprs[0].is_rank) unsupported("WindowExec: a group limit over an aggregate window column is not on the GPU path (rank-like functions are)");
+  }
+  n->schema = in;                                                             // WindowContext::try_new: input ++ window fields
+  if (n->output_window_cols) for (auto& w : n->window_exprs) n->schema.fields.push_back(w.field);
+  return n;
+}
+
 // the `~TABLE` column the reference appends to the build side's batches (joins/join_hash_map.rs:409-431, 459-465)
 SchemaDef join_hash_map_schema(const SchemaDef& data) {
   SchemaDef s = data;
@@ -714,8 +816,9 @@ PlanP parse_plan(Reader r) {                  // PhysicalPlanNode oneof (auron.p
       case 16: return parse_agg(r.bytes());
       case 18: return parse_leaf(r.bytes(), true);
       case 20: return parse_expand(r.bytes());
+      case 22: return parse_window(r.bytes());
       case 1: case 3: case 4: case 9: case 10: case 14: case 17: case 19:
-      case 21: case 22: case 23: case 24: case 25:
+      case 21: case 23: case 24: case 25:
         unsupported("plan node #" + std::to_string(f) + " is outside the Filter/Project/Agg hot path (SURVEY.md §8)");
       default: r.skip(wt);
     }
@@ -803,6 +906,26 @@ static void explain_rec(const PlanP& p, int depth, std::ostringstream& o) {
         o << "]";
       }
       o << "] schema=" << schema_str(p->schema) << "\n"; break;
+    }
+    case N_WINDOW: {
+      static const char* rank_names[] = {"row_number", "rank", "dense_rank"};
+      static const char* agg_names[] = {"MIN", "MAX", "SUM", "AVG", "COUNT"};
+      o << ind << "WindowExec: [";
+      for (size_t i = 0; i < p->window_exprs.size(); i++) {
+        const auto& w = p->window_exprs[i];
+        o << (i ? ", " : "");
+        if (w.is_rank) o << rank_names[w.rank_fn] << "()";
+        else { o << agg_names[w.agg.fn] << "("; for (size_t j = 0; j < w.agg.args.size(); j++) o << (j ? ", " : "") << explain_expr(w.agg.args[j]); o << ")"; }
+        o << " AS " << w.field.name << ":" << w.field.type.str();
+      }
+      o << "] partition_by=[";
+      for (size_t i = 0; i < p->window_partition.size(); i++) o << (i ? ", " : "") << explain_expr(p->window_partition[i]);
+      o << "] order_by=[";
+      for (size_t i = 0; i < p->window_order.size(); i++) o << (i ? ", " : "") << explain_expr(p->window_order[i].expr) << (p->window_order[i].asc ? " ASC" : " DESC") << (p->window_order[i].nulls_first ? " NULLS FIRST" : " NULLS LAST");
+      o << "]";
+      if (p->window_has_limit) o << " group_limit=" << p->window_limit;
+      o << " output_window_cols=" << (p->output_window_cols ? "true" : "false") << "\n";
+      break;
     }
     case N_SORT: {
       o << ind << "SortExec [";

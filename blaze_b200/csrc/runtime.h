@@ -123,12 +123,20 @@ void set_file_reader(b200q_file_reader_fn fn, void* ctx);
 // SortExec (sort_stage.cu): collects its input, emits the sorted (and `fetch`-limited) rows at finish
 std::unique_ptr<Stage> make_sort_stage(OpContext& cx, const SchemaDef& in_schema, const PlanNode& node);
 
+// WindowExec (window_stage.cu): partition / order keys and aggregate arguments are input columns, by index; the output is the
+// first `n_fwd` input columns ++ one column per window expression (the trailing input columns are dropped)
+struct WindowCols { std::vector<int> partition_cols, order_cols; std::vector<std::vector<int>> agg_args; size_t n_fwd = 0; };
+std::unique_ptr<Stage> make_window_stage(OpContext& cx, const SchemaDef& in_schema, const PlanNode& node, const WindowCols& cols);
+
 // Hash join (join_stage.cu): the build side is its own op; probe ops attach to its result
 struct JoinBuilt;
 std::unique_ptr<Stage> make_join_build_stage(OpContext& cx, const SchemaDef& in_schema, const PlanNode& node);
 std::unique_ptr<Stage> make_join_probe_stage(OpContext& cx, const SchemaDef& in_schema, const PlanNode& node);
 struct JoinBuildResult { virtual ~JoinBuildResult() {} virtual std::shared_ptr<JoinBuilt> built() const = 0; };
 struct JoinProbeAttach { virtual ~JoinProbeAttach() {} virtual void attach(std::shared_ptr<JoinBuilt> b) = 0; };
+
+// a column as the kernels see it (stages.cu)
+DevCol dev_col_of(const DevColumn& c);
 
 // helpers of the C ABI layer (capi.cu) shared with exchange.cu
 DType type_of_format(const char* arrow_format);

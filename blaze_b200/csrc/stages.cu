@@ -62,7 +62,7 @@ DevMemP DevMem::borrow(const void* p, size_t bytes, std::shared_ptr<void> owner)
 
 static inline size_t bitmap_bytes(int64_t n) { return (size_t)((n + 31) / 32) * 4; }
 
-static DevCol dev_col_of(const DevColumn& c) {
+DevCol dev_col_of(const DevColumn& c) {
   DevCol d{};
   const int w = c.type.byte_width();
   d.values = c.values ? (const uint8_t*)c.values->ptr + (size_t)c.offset * (size_t)w : nullptr;

@@ -312,6 +312,40 @@ class AggFunctionExpr:
         object.__setattr__(self, "return_type", return_type)
 
 
+# WindowFunction / WindowFunctionType (auron.proto:121-125, 556-559)
+ROW_NUMBER, RANK, DENSE_RANK = 0, 1, 2
+WINDOW_FUNC, WINDOW_AGG = 0, 1
+
+
+@dataclass(frozen=True)
+class WindowExpr:
+    """`WindowExprNode{field, return_type, func_type, window_func, agg_func, children}` — WindowExpr::new(func, children,
+    field, return_type) (datafusion-ext-plans/src/window/mod.rs).  Rank-like: func_type WINDOW_FUNC, window_func one of
+    ROW_NUMBER / RANK / DENSE_RANK; aggregates: func_type WINDOW_AGG, agg_func an AGG_* code over `children`."""
+    field: "T.Field"
+    func_type: int
+    window_func: int = ROW_NUMBER
+    agg_func: int = 0
+    children: Tuple[Expr, ...] = ()
+    return_type: Optional[DataType] = None
+
+    def __init__(self, field, func_type, window_func=ROW_NUMBER, agg_func=0, children=(), return_type=None):
+        object.__setattr__(self, "field", field)
+        object.__setattr__(self, "func_type", func_type)
+        object.__setattr__(self, "window_func", window_func)
+        object.__setattr__(self, "agg_func", agg_func)
+        object.__setattr__(self, "children", tuple(children))
+        object.__setattr__(self, "return_type", return_type if return_type is not None else field.dtype)
+
+    @classmethod
+    def rank_like(cls, name: str, window_func: int, nullable: bool = False):
+        return cls(T.Field(name, T.int32, nullable), WINDOW_FUNC, window_func=window_func)
+
+    @classmethod
+    def agg(cls, name: str, agg_func: int, children, return_type: DataType, nullable: bool = True):
+        return cls(T.Field(name, return_type, nullable), WINDOW_AGG, agg_func=agg_func, children=children, return_type=return_type)
+
+
 @dataclass(frozen=True)
 class GroupingExpr:
     field_name: str

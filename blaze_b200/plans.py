@@ -250,6 +250,35 @@ class SortExec(ExecutionPlan):
         return P.sort_node(self.input.node(), [(e, not d, nf) for e, d, nf in self.exprs], self.fetch)      # wire: asc = !descending (from_proto.rs:240-246)
 
 
+class WindowExec(ExecutionPlan):
+    """WindowExec::try_new(input, window_exprs, partition_spec, order_spec, group_limit, output_window_cols)
+    (window_exec.rs:65-87): running row_number / rank / dense_rank and SUM / AVG / MIN / MAX / COUNT over ROWS BETWEEN UNBOUNDED
+    PRECEDING AND CURRENT ROW of input sorted by (partition_spec, order_spec).  order_spec = [(expr, descending, nulls_first)] as
+    in SortExec.  A group limit k (WindowGroupLimitExec) keeps the rows whose one window column is <= k as i32."""
+
+    def __init__(self, input: ExecutionPlan, window_exprs: Sequence[E.WindowExpr], partition_spec: Sequence[E.Expr], order_spec,
+                 group_limit: Optional[int] = None, output_window_cols: bool = True):
+        self.input, self.window_exprs, self.partition_spec = input, list(window_exprs), list(partition_spec)
+        self.order_spec = [(e, bool(d), bool(nf)) for e, d, nf in order_spec]
+        self.group_limit, self.output_window_cols = group_limit, bool(output_window_cols)
+        self._validate()
+
+    try_new = classmethod(lambda cls, *a, **k: cls(*a, **k))
+
+    def schema(self):
+        fields = list(self.input.schema())
+        if self.output_window_cols:
+            fields += [w.field for w in self.window_exprs]
+        return Schema(fields)
+
+    def children(self):
+        return [self.input]
+
+    def node(self):
+        return P.window_node(self.input.node(), self.window_exprs, self.partition_spec, [(e, not d, nf) for e, d, nf in self.order_spec],
+                             self.group_limit, self.output_window_cols)
+
+
 # protobuf JoinType (auron.proto:475-483): SEMI / ANTI are the Left forms (auron-serde/src/lib.rs:104-116)
 JOIN_INNER, JOIN_LEFT, JOIN_RIGHT, JOIN_FULL, JOIN_SEMI, JOIN_ANTI, JOIN_EXISTENCE = range(7)
 LEFT_SIDE, RIGHT_SIDE = 0, 1

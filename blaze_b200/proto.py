@@ -178,6 +178,7 @@ def _build_pool():
         ("broadcast_join", 13, "BroadcastJoinExecNode", O), ("filter", 8, "FilterExecNode", O),
         ("empty_partitions", 15, "EmptyPartitionsExecNode", O), ("agg", 16, "AggExecNode", O),
         ("ffi_reader", 18, "FFIReaderExecNode", O), ("expand", 20, "PhysicalPlanNode.ExpandExecNode", O),
+        ("window", 22, "PhysicalPlanNode.WindowExecNode", O),
     ], oneofs=["PhysicalPlanType"])
     # ExpandExecNode{input=1, schema=2, projections=3} and ExpandProjection{expr=1} (auron.proto:714-722) are top-level in the reference;
     # nested here like the string-match nodes above (same bytes on the wire), the top-level set stays that of the field table of
@@ -186,6 +187,22 @@ def _build_pool():
     _msg(fd, "ExpandExecNode", [("input", 1, "PhysicalPlanNode"), ("schema", 2, "Schema"), ("projections", 3, "PhysicalPlanNode.ExpandProjection", R)],
          into=pp.nested_type)
     _msg(fd, "ExpandProjection", [("expr", 1, "PhysicalExprNode", R)], into=pp.nested_type)
+    # WindowExecNode, WindowExprNode, WindowGroupLimit and the WindowFunction / WindowFunctionType enums (auron.proto:121-125,
+    # 537-562): nested the same way; tests/test_proto_window_compat.py checks them against tests/golden/auron_proto_window_fields.json
+    for name, values in (("WindowFunction", [("ROW_NUMBER", 0), ("RANK", 1), ("DENSE_RANK", 2)]), ("WindowFunctionType", [("Window", 0), ("Agg", 1)])):
+        e = pp.enum_type.add()
+        e.name = name
+        for vn, vv in values:
+            ev = e.value.add()
+            ev.name, ev.number = vn, vv
+    _msg(fd, "WindowExecNode", [("input", 1, "PhysicalPlanNode"), ("window_expr", 2, "PhysicalPlanNode.WindowExprNode", R),
+                                ("partition_spec", 3, "PhysicalExprNode", R), ("order_spec", 4, "PhysicalExprNode", R),
+                                ("group_limit", 5, "PhysicalPlanNode.WindowGroupLimit"), ("output_window_cols", 6, _F.TYPE_BOOL)],
+         into=pp.nested_type)
+    _msg(fd, "WindowExprNode", [("field", 1, "Field"), ("return_type", 1000, "ArrowType"), ("func_type", 2, "enum:PhysicalPlanNode.WindowFunctionType"),
+                                ("window_func", 3, "enum:PhysicalPlanNode.WindowFunction"), ("agg_func", 4, "enum:AggFunction"),
+                                ("children", 5, "PhysicalExprNode", R)], into=pp.nested_type)
+    _msg(fd, "WindowGroupLimit", [("k", 1, _F.TYPE_UINT32)], into=pp.nested_type)
     _msg(fd, "PartitionId", [("stage_id", 2, _F.TYPE_UINT32), ("partition_id", 4, _F.TYPE_UINT32), ("task_id", 5, _F.TYPE_UINT64)])
     _msg(fd, "TaskDefinition", [("task_id", 1, "PartitionId"), ("plan", 2, "PhysicalPlanNode")])
 
@@ -380,6 +397,31 @@ def expand_node(input_node, schema: Schema, projections):
         p = n.expand.projections.add()
         for e in proj:
             p.expr.add().CopyFrom(expr_msg(e))
+    return n
+
+
+def window_node(input_node, window_exprs, partition_spec, order_spec, group_limit=None, output_window_cols=True):
+    """order_spec: [(expr, asc, nulls_first)], each sent as a PhysicalSortExprNode (from_proto.rs:621-652)"""
+    n = PhysicalPlanNode()
+    w = n.window
+    w.input.CopyFrom(input_node)
+    for we in window_exprs:
+        x = w.window_expr.add()
+        x.field.name, x.field.nullable = we.field.name, we.field.nullable
+        x.field.arrow_type.CopyFrom(arrow_type_msg(we.field.dtype))
+        x.return_type.CopyFrom(arrow_type_msg(we.return_type))
+        x.func_type, x.window_func, x.agg_func = we.func_type, we.window_func, we.agg_func
+        for c in we.children:
+            x.children.add().CopyFrom(expr_msg(c))
+    for e in partition_spec:
+        w.partition_spec.add().CopyFrom(expr_msg(e))
+    for e, asc, nulls_first in order_spec:
+        x = w.order_spec.add()
+        x.sort.expr.CopyFrom(expr_msg(e))
+        x.sort.asc, x.sort.nulls_first = asc, nulls_first
+    if group_limit is not None:
+        w.group_limit.k = group_limit
+    w.output_window_cols = output_window_cols
     return n
 
 

@@ -468,3 +468,76 @@ if any(t in (ONLY or "E1,E2") for t in ("E1", "E2")):
                         "E2 Filter -> Expand ROLLUP(k1, k2) -> Filter(all rows) -> AggExec(Partial) -> AggExec(Final), standalone Expand",
                         fin, e_spec, [ef, ek1, ek2, ev], native.default_conf(agg_initial_groups=1 << 20), erows, 3)
     del ef, ek1, ek2, ev
+
+
+# W1: WindowExec over 2^28 pre-sorted device rows: p = row >> 8 (2^20 partitions of 256 rows), o = (row & 255) >> 2 (peer groups of 4),
+# non-null int64 v; row_number, rank, dense_rank, SUM(v), COUNT(v).  Kernel time = the window kernels' events (flags + one reduce-then-scan
+# per function): every key and argument is an input column (SUM's TryCast to int64 is v itself), so the window stage is the op's first stage
+# and hot_kernel_ns is exactly its events.  Algorithmic bytes: 24 B read (p, o, v) + 28 B written (3 x int32 + 2 x int64) per row.  Results are checked against torch
+# after the timed region.
+# W2: SortExec(p, o) -> WindowExec(rank, group limit 100) over 2^26 rows, p ~ U[0, 2^16), o ~ U[0, 1000) (the q67 shape), timed as
+# whole-op wall time push_device -> finish -> sync; the number of surviving rows is checked against torch.
+def cuda_col(o, i, nbytes, dtype):
+    return torch.as_tensor(__import__("bench").CudaView(o.array.children[i].contents.buffers[1], nbytes, o), device="cuda").view(dtype)
+
+
+if any(t in (ONLY or "W1,W2") for t in ("W1", "W2")):
+    import time
+    w_sch = T.Schema([T.Field(nm, T.int64, False) for nm in ("p", "o", "v")])
+    part, order = [E.Column("p")], [(E.Column("o"), False, True)]
+    wx = lambda nm, f: E.WindowExpr.rank_like(nm, f)
+    if "W1" in (ONLY or "W1"):
+        idx = torch.arange(rows, dtype=torch.int64, device=dev)
+        wp, wo = idx >> 8, (idx & 255) >> 2
+        wv = torch.randint(-10**6, 10**6, (rows,), dtype=torch.int64, device=dev, generator=g)
+        w1 = PL.WindowExec(PL.MemoryExec(w_sch), [wx("rn", E.ROW_NUMBER), wx("rk", E.RANK), wx("dr", E.DENSE_RANK),
+                                                   E.WindowExpr.agg("s", E.AGG_SUM, [E.Column("v")], T.int64), E.WindowExpr.agg("c", E.AGG_COUNT, [E.Column("v")], T.int64, False)], part, order)
+        best = None
+        for _ in range(REPS or 3):
+            with native.NativeOp(w1.plan_bytes(), native.default_conf(), 0) as op:
+                op.push_device(native.DeviceBatch([(t.data_ptr(), 0, rows) for t in (wp, wo, wv)], rows, 0, keepalive=(wp, wo, wv)))
+                op.finish()
+                o = op.pull_device()
+                m = op.metrics()
+                if best is None or m["hot_kernel_ns"] < best[0]:
+                    pos = idx & 255
+                    cs = torch.cumsum(wv.view(-1, 256), 1).view(-1)
+                    ok = bool((cuda_col(o, 3, rows * 4, torch.int32) == (pos + 1).int()).all()) and bool((cuda_col(o, 4, rows * 4, torch.int32) == ((pos >> 2) * 4 + 1).int()).all()) \
+                        and bool((cuda_col(o, 5, rows * 4, torch.int32) == ((pos >> 2) + 1).int()).all()) and bool((cuda_col(o, 6, rows * 8, torch.int64) == cs).all()) \
+                        and bool((cuda_col(o, 7, rows * 8, torch.int64) == pos + 1).all())
+                    best = (m["hot_kernel_ns"], m, ok)
+                native.release_device_array(o)
+        t, m, ok = best
+        gbs = 52.0 * rows / t
+        print(json.dumps({"shape": "W1 WindowExec row_number, rank, dense_rank, SUM, COUNT over 2^20 partitions", "rows": rows, "verified": ok,
+                          "window_kernel_ms": t / 1e6, "rows_per_s": rows / (t * 1e-9), "alg_GBps": gbs, "frac_of_hbm_peak": gbs / peak,
+                          "launches": m["gpu_kernel_launches"]}), flush=True)
+        del idx, wp, wo, wv, cs, pos
+        torch.cuda.empty_cache()
+    if "W2" in (ONLY or "W2"):
+        n2 = int(os.environ.get("ROWS", 1 << 26))
+        wp = torch.randint(0, 1 << 16, (n2,), dtype=torch.int64, device=dev, generator=g)
+        wo = torch.randint(0, 1000, (n2,), dtype=torch.int64, device=dev, generator=g)
+        wv = torch.randint(-10**6, 10**6, (n2,), dtype=torch.int64, device=dev, generator=g)
+        w2 = PL.WindowExec(PL.SortExec(PL.MemoryExec(w_sch), [(E.Column("p"), False, True), (E.Column("o"), False, True)]), [wx("rk", E.RANK)], part, order, 100, False)
+        best = None
+        for _ in range(REPS or 3):
+            with native.NativeOp(w2.plan_bytes(), native.default_conf(), 0) as op:
+                torch.cuda.synchronize(); t0 = time.perf_counter()
+                op.push_device(native.DeviceBatch([(t.data_ptr(), 0, n2) for t in (wp, wo, wv)], n2, 0, keepalive=(wp, wo, wv)))
+                op.finish(); op.sync()
+                dt = time.perf_counter() - t0
+                m = op.metrics(); n_out = 0
+                while True:
+                    o = op.pull_device()
+                    if o is None: break
+                    n_out += o.array.length; native.release_device_array(o)
+            if best is None or dt < best[0]: best = (dt, m, n_out)
+        dt, m, n_out = best
+        key, _ = torch.sort(wp * 1024 + wo)
+        i2 = torch.arange(n2, device=dev)
+        pstart = torch.cummax(torch.where(torch.cat([torch.ones(1, dtype=torch.bool, device=dev), (key[1:] >> 10) != (key[:-1] >> 10)]), i2, 0), 0).values
+        head = torch.cummax(torch.where(torch.cat([torch.ones(1, dtype=torch.bool, device=dev), key[1:] != key[:-1]]), i2, 0), 0).values
+        expect = int(((head - pstart + 1) <= 100).sum())
+        print(json.dumps({"shape": "W2 SortExec(p, o) -> WindowExec(rank, group limit 100)", "rows": n2, "out_rows": n_out, "verified": n_out == expect,
+                          "wall_ms_push_to_sync": dt * 1e3, "rows_per_s": n2 / dt, "launches": m["gpu_kernel_launches"]}), flush=True)
