@@ -172,16 +172,18 @@ __global__ void __launch_bounds__(JB) join_mark_build_kernel(long long n, const 
 // (probe row, build row) pairs — no per-row intermediates, no global scan.  The output rows of a tile are contiguous and
 // come from a contiguous input range, so the gathers that follow stay inside a 16 KB window per column; the order is not a contract.
 // pidx == null: only count (cursor += matches), for build sides with duplicated keys whose output size is not bounded by n.
+// The sums are 64-bit: one key may have up to 2^30 rows, so a thread's 8 rows can reach 2^33 and a tile 2^41.  In 32 bits a
+// tile of 2048 rows of a 2^21-row key wraps to 0 and the caller sees no output instead of refusing the batch.
 constexpr int JP_ROWS = 8;
 __global__ void __launch_bounds__(JB) join_probe_pairs_kernel(const JoinKeys k, long long n, const JoinTable t, int probe_outer, unsigned long long* cursor,
                                                               uint32_t* __restrict__ pidx, uint32_t* __restrict__ bidx, uint8_t* mark) {
-  __shared__ unsigned s_warp[JB / 32];
+  __shared__ unsigned long long s_warp[JB / 32];
   __shared__ unsigned long long s_base;
   const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const long long ntiles = (n + JB * JP_ROWS - 1) / (JB * JP_ROWS);
   for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const long long t0 = tile * (JB * JP_ROWS);
-    uint32_t h[JP_ROWS]; unsigned c[JP_ROWS]; unsigned mine = 0;
+    uint32_t h[JP_ROWS]; unsigned c[JP_ROWS]; unsigned long long mine = 0;
 #pragma unroll
     for (int r = 0; r < JP_ROWS; r++) {
       const long long i = t0 + r * JB + threadIdx.x;
@@ -193,13 +195,13 @@ __global__ void __launch_bounds__(JB) join_probe_pairs_kernel(const JoinKeys k, 
       }
       mine += c[r];
     }
-    unsigned inc = mine;
+    unsigned long long inc = mine;
 #pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const unsigned o = __shfl_up_sync(0xFFFFFFFFu, inc, d); if (lane >= d) inc += o; }
+    for (int d = 1; d < 32; d <<= 1) { const unsigned long long o = __shfl_up_sync(0xFFFFFFFFu, inc, d); if (lane >= d) inc += o; }
     if (lane == 31) s_warp[warp] = inc;
     __syncthreads();
-    unsigned before = 0, total = 0;
-    for (int w = 0; w < JB / 32; w++) { const unsigned v = s_warp[w]; if (w < (int)warp) before += v; total += v; }
+    unsigned long long before = 0, total = 0;
+    for (int w = 0; w < JB / 32; w++) { const unsigned long long v = s_warp[w]; if (w < (int)warp) before += v; total += v; }
     if (threadIdx.x == 0 && total) s_base = atomicAdd(cursor, (unsigned long long)total);
     __syncthreads();
     if (pidx && mine) {
