@@ -52,6 +52,12 @@ __device__ __forceinline__ void emit_row_columns(const EmitTable& emit, unsigned
           emit_store(ec, at, valid ? f64_bits(avg_f64_final(sum, cnt)) : 0, 0, valid);
           break;
         }
+        case EMIT_FIRST_VALUE: {
+          const bool valid = slot[ec.word2] != ~0ULL && (ec.vbit == 0xFF || ((flags >> ec.vbit) & 1));
+          emit_store(ec, at, valid ? slot[ec.word] : 0, (valid && ec.phys == PH_DEC128) ? slot[ec.word + 1] : 0, valid);
+          break;
+        }
+        case EMIT_FIRST_FLAG: emit_store(ec, at, slot[ec.word2] != ~0ULL ? 1 : 0, 0, true); break;
         default: {   // EMIT_AVG_DEC: i128::checked_div_euclid(sum, count) (avg.rs:158-165)
           const long long cnt = (long long)slot[ec.word2];
           const bool valid = (ec.vbit == 0xFF ? true : ((flags >> ec.vbit) & 1)) && cnt != 0;

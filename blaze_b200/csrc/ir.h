@@ -86,14 +86,14 @@ struct Expr {
   std::vector<ExprP> children;
 };
 
-enum AggFn : uint8_t { AGG_MIN = 0, AGG_MAX = 1, AGG_SUM = 2, AGG_AVG = 3, AGG_COUNT = 4 };
+enum AggFn : uint8_t { AGG_MIN = 0, AGG_MAX = 1, AGG_SUM = 2, AGG_AVG = 3, AGG_COUNT = 4, AGG_FIRST = 7, AGG_FIRST_IGNORES_NULL = 8 };
 enum AggMode : uint8_t { MODE_PARTIAL = 0, MODE_PARTIAL_MERGE = 1, MODE_FINAL = 2 };
 
 struct AggDef {
   AggFn fn;
   AggMode mode;
   std::string field_name;
-  DType data_type;              // Agg::data_type(): Sum/Avg = return_type, Min/Max = child type, Count = Int64
+  DType data_type;              // Agg::data_type(): Sum/Avg = return_type, Min/Max/First = child type, Count = Int64
   std::vector<ExprP> args;      // after create_agg rewriting: Sum/Avg -> TryCast(child,rt); Count -> nullable children only
   bool nullable() const { return fn != AGG_COUNT; }
   DType final_type() const {    // type of the Final-mode output column

@@ -463,8 +463,39 @@ __device__ __forceinline__ void acc_apply(uint8_t kind, unsigned long long* ke, 
   }
 }
 
+// FIRST / FIRST_IGNORES_NULL: the row's value replaces the slot's when the row's arrival ordinal is smaller.  The ordinal of
+// a slot only ever decreases, so a relaxed load that already shows a smaller one ends the work with no atomic (every row
+// that is not its group's earliest so far); otherwise the slot lock of the 128-bit MIN / MAX makes the re-check and the
+// writes of ordinal, value words and validity bit one step.  The FIRST accumulators of one aggregate share the ordinal
+// word: the earliest row writes each of them in its own lock hold, and `<=` lets it pass the ordinal it wrote itself.
+// Returns false when a smaller ordinal was seen (the caller skips the other accumulators on that ordinal word).
+__device__ __forceinline__ bool first_apply(unsigned long long* ke, unsigned long long* ae, const AccOp& a, const uint64_t* arg, bool arg_valid, uint64_t ord) {
+  if (ld_relaxed_u64(ae + a.oword) < ord) return false;
+  unsigned* flags = (unsigned*)ke + 1;
+  while (atomicOr(flags, FLAG_SLOT_LOCK) & FLAG_SLOT_LOCK) {}
+  __threadfence();
+  volatile unsigned long long* p = ae;
+  const bool win = ord <= p[a.oword];
+  if (win) {
+    p[a.oword] = ord;
+    p[a.word] = arg[0];
+    if (a.nwords == 2) p[a.word + 1] = arg[1];
+    if (a.vbit != 0xFF) { if (arg_valid) atomicOr(flags, 1u << a.vbit); else atomicAnd(flags, ~(1u << a.vbit)); }
+  }
+  __threadfence();
+  atomicAnd(flags, ~FLAG_SLOT_LOCK);
+  return win;
+}
+
+// eligibility of a row for a FIRST accumulator (`o0`: value output, `o1`: flag output or AGG_NO_ARG; validity bits in `vb`)
+__device__ __forceinline__ bool first_eligible(const AccOp& a, const AggLayout& lay, const uint64_t* buf, uint32_t vb, int o0, int o1) {
+  if (a.kind == ACC_FIRST_VALID) return o0 != AGG_NO_ARG && ((vb >> o0) & 1);                // first_ignores_null.rs: a valid value
+  if (o1 == AGG_NO_ARG) return true;                                                        // first.rs update: any row
+  return ((vb >> o1) & 1) && buf[lay.out_word[o1]] != 0;                                    // first.rs merge: the state's flag is set
+}
+
 // find-or-insert the key, then apply every accumulator update; returns false when the row had to be deferred
-__device__ __forceinline__ bool agg_upsert(const AggLayout& lay, const AggTable& tab, const uint64_t* buf, uint32_t vb) {
+__device__ __forceinline__ bool agg_upsert(const AggLayout& lay, const AggTable& tab, const uint64_t* buf, uint32_t vb, uint64_t ord) {
   uint64_t kw[AGG_MAX_KEYS * 2];
   uint32_t knull;
   const uint64_t h = hash_keys(lay, buf, vb, knull, kw);
@@ -476,10 +507,16 @@ __device__ __forceinline__ bool agg_upsert(const AggLayout& lay, const AggTable&
   unsigned long long* const ke = tab.keys + slot * (uint64_t)lay.kstride;
   unsigned long long* const ae = tab.accs + slot * (uint64_t)lay.astride;
   // accumulate (K6 / K7)
+  int lost = -1;                           // ordinal word on which this row already lost to an earlier row
   for (int j = 0; j < lay.nacc; j++) {
     const AccOp a = lay.acc[j];
     const int o = a.arg_out[0];
     const uint64_t* arg = buf + lay.out_word[o];
+    if (acc_is_first(a.kind)) {
+      if (a.oword != lost && first_eligible(a, lay, buf, vb, o, a.nargs > 1 ? a.arg_out[1] : AGG_NO_ARG) &&
+          !first_apply(ke, ae, a, arg, (vb >> o) & 1, ord)) lost = a.oword;
+      continue;
+    }
     bool valid = true;
     for (int i = 0; i < a.nargs; i++) valid = valid && ((vb >> a.arg_out[i]) & 1);
     if (!valid) continue;
@@ -490,7 +527,7 @@ __device__ __forceinline__ bool agg_upsert(const AggLayout& lay, const AggTable&
 }
 
 // agg_upsert for one grouping set: constant keys come from the set's descriptor, arguments from the set's VM outputs
-__device__ __forceinline__ bool agg_upsert_set(const AggLayout& lay, const AggTable& tab, const uint64_t* buf, uint32_t vb, const AggSetDesc* __restrict__ sd) {
+__device__ __forceinline__ bool agg_upsert_set(const AggLayout& lay, const AggTable& tab, const uint64_t* buf, uint32_t vb, const AggSetDesc* __restrict__ sd, uint64_t ord) {
   uint64_t kw[AGG_MAX_KEYS * 2];
   uint32_t knull = 0;
   int w = 0;
@@ -515,9 +552,17 @@ __device__ __forceinline__ bool agg_upsert_set(const AggLayout& lay, const AggTa
   unsigned long long* const ke = tab.keys + slot * (uint64_t)lay.kstride;
   unsigned long long* const ae = tab.accs + slot * (uint64_t)lay.astride;
   const uint32_t skip = sd->acc_skip;
+  int lost = -1;
   for (int j = 0; j < lay.nacc; j++) {
     if ((skip >> j) & 1) continue;
     const AccOp a = lay.acc[j];
+    if (acc_is_first(a.kind)) {            // a value that is a NULL literal in this set is AGG_NO_ARG: a NULL value
+      const int o = sd->acc_arg[j][0];
+      const bool ov = o != AGG_NO_ARG && ((vb >> o) & 1);
+      if (a.oword != lost && first_eligible(a, lay, buf, vb, o, sd->acc_arg[j][1]) &&
+          !first_apply(ke, ae, a, buf + lay.out_word[o == AGG_NO_ARG ? 0 : o], ov, ord)) lost = a.oword;
+      continue;
+    }
     bool valid = true;
     for (int i = 0; i < 4; i++) { const int o = sd->acc_arg[j][i]; if (o != AGG_NO_ARG) valid = valid && ((vb >> o) & 1); }
     if (!valid) continue;
@@ -529,7 +574,8 @@ __device__ __forceinline__ bool agg_upsert_set(const AggLayout& lay, const AggTa
 }
 
 __global__ void __launch_bounds__(AG_BLOCK) agg_update_kernel(const VmProgram* __restrict__ prog, const ColTable cols, const AggLayout lay, const AggTable tab,
-                                                              long long row_begin, long long n, const uint32_t* __restrict__ row_list) {
+                                                              long long row_begin, long long n, const uint32_t* __restrict__ row_list,
+                                                              unsigned long long ord_base) {
   __shared__ VmInstr s_code[VM_MAX_CODE];
   __shared__ uint64_t s_pool[VM_MAX_POOL];
   load_program(prog, s_code, s_pool);
@@ -553,7 +599,7 @@ __global__ void __launch_bounds__(AG_BLOCK) agg_update_kernel(const VmProgram* _
     vm_run<AG_R>(s_code, s_pool, 0, cols, row, inb, alive, err, sink);
 #pragma unroll
     for (int r = 0; r < AG_R; r++) {
-      if (alive[r] && !agg_upsert(lay, tab, buf[r], vb[r])) {
+      if (alive[r] && !agg_upsert(lay, tab, buf[r], vb[r], ord_base + (unsigned long long)row[r])) {
         const unsigned long long at = atomicAdd(tab.counters + 1, 1ULL);
         tab.deferred[at] = rel[r];
       }
@@ -565,7 +611,7 @@ __global__ void __launch_bounds__(AG_BLOCK) agg_update_kernel(const VmProgram* _
 // row * nsets + set and replays that set only, so sets of the row that already landed are not counted twice.
 __global__ void __launch_bounds__(AG_BLOCK) agg_update_sets_kernel(const VmProgram* __restrict__ prog, const ColTable cols, const AggLayout lay, const AggTable tab,
                                                                    long long row_begin, long long n, const uint32_t* __restrict__ row_list,
-                                                                   const AggSetDesc* __restrict__ sets, int nsets) {
+                                                                   const AggSetDesc* __restrict__ sets, int nsets, unsigned long long ord_base) {
   __shared__ VmInstr s_code[VM_MAX_CODE];
   __shared__ uint64_t s_pool[VM_MAX_POOL];
   load_program(prog, s_code, s_pool);
@@ -594,7 +640,7 @@ __global__ void __launch_bounds__(AG_BLOCK) agg_update_sets_kernel(const VmProgr
       if (!alive[r]) continue;
       const int s0 = only[r] < 0 ? 0 : only[r], s1 = only[r] < 0 ? nsets : only[r] + 1;
       for (int s = s0; s < s1; s++) {
-        if (!agg_upsert_set(lay, tab, buf[r], vb[r], sets + s)) {
+        if (!agg_upsert_set(lay, tab, buf[r], vb[r], sets + s, (ord_base + (unsigned long long)row[r]) * (unsigned)nsets + (unsigned)s)) {
           const unsigned long long at = atomicAdd(tab.counters + 1, 1ULL);
           tab.deferred[at] = rel[r] * (uint32_t)nsets + (uint32_t)s;
         }
@@ -610,18 +656,18 @@ static int grid_for(int64_t ntiles, int per_sm) {
 }
 
 int launch_agg_update(const VmProgram* d_prog, const ColTable& cols, const AggLayout& lay, const AggTable& tab, int64_t row_begin, int64_t n,
-                      const uint32_t* d_row_list, cudaStream_t s) {
+                      const uint32_t* d_row_list, uint64_t ord_base, cudaStream_t s) {
   if (n <= 0) return 0;
   const int64_t ntiles = (n + AG_TILE - 1) / AG_TILE;
-  agg_update_kernel<<<grid_for(ntiles, 8), AG_BLOCK, 0, s>>>(d_prog, cols, lay, tab, row_begin, n, d_row_list);
+  agg_update_kernel<<<grid_for(ntiles, 8), AG_BLOCK, 0, s>>>(d_prog, cols, lay, tab, row_begin, n, d_row_list, ord_base);
   return 1;
 }
 
 int launch_agg_update_sets(const VmProgram* d_prog, const ColTable& cols, const AggLayout& lay, const AggTable& tab, int64_t row_begin, int64_t n,
-                           const uint32_t* d_row_list, const AggSetDesc* d_sets, int nsets, cudaStream_t s) {
+                           const uint32_t* d_row_list, const AggSetDesc* d_sets, int nsets, uint64_t ord_base, cudaStream_t s) {
   if (n <= 0) return 0;
   const int64_t ntiles = (n + AG_TILE - 1) / AG_TILE;
-  agg_update_sets_kernel<<<grid_for(ntiles, 8), AG_BLOCK, 0, s>>>(d_prog, cols, lay, tab, row_begin, n, d_row_list, d_sets, nsets);
+  agg_update_sets_kernel<<<grid_for(ntiles, 8), AG_BLOCK, 0, s>>>(d_prog, cols, lay, tab, row_begin, n, d_row_list, d_sets, nsets, ord_base);
   return 1;
 }
 
@@ -733,6 +779,7 @@ __global__ void __launch_bounds__(256) frozen_lengths_kernel(const FrozenTable f
     for (int k = 0; k < ft.nfields; k++) {
       const FrozenField& f = ft.f[k];
       if (f.kind == FZ_COUNT) len += varint_len(((const unsigned long long*)f.values)[i]);
+      else if (f.kind == FZ_BOOL) len += 1;
       else len += 1 + ((f.valid ? f.valid[i] != 0 : true) ? f.width : 0);
     }
     lengths[i] = len;
@@ -748,6 +795,9 @@ __global__ void __launch_bounds__(256) frozen_write_kernel(const FrozenTable ft,
         unsigned long long v = ((const unsigned long long*)f.values)[i];           // write_len (io/mod.rs:60-68)
         while (v >= 128) { *p++ = (uint8_t)(128 + (v & 127)); v >>= 7; }
         *p++ = (uint8_t)v;
+      } else if (f.kind == FZ_BOOL) {                                              // acc.rs:180-190
+        const uint8_t v = ((const uint8_t*)f.values)[i] != 0;
+        *p++ = f.valid ? (f.valid[i] ? 1 + v : 0) : (v ? 2 : 0);
       } else {
         const bool valid = f.valid ? f.valid[i] != 0 : true;
         *p++ = valid ? 1 : 0;                                                      // acc.rs:335-346
@@ -777,6 +827,11 @@ __global__ void __launch_bounds__(256) frozen_read_kernel(const FrozenTable ft, 
           v += (unsigned long long)(b - 128) << shift; shift += 7;
         }
         ((unsigned long long*)f.values)[i] = v;
+      } else if (f.kind == FZ_BOOL) {                                              // acc.rs:193-207
+        if (p >= end) { atomicOr(err, 4); break; }
+        const uint8_t b = *p++;
+        if (f.valid) { ((uint8_t*)f.valid)[i] = b != 0; ((uint8_t*)f.values)[i] = b > 1; }
+        else ((uint8_t*)f.values)[i] = b != 0;                                     // FIRST's flag: any non-zero byte is set
       } else {                                                                     // acc.rs:349-365
         if (p >= end) { atomicOr(err, 4); break; }
         const bool valid = *p++ == 1;

@@ -21,14 +21,22 @@ enum AccKind : uint8_t {
   ACC_MIN_I64, ACC_MAX_I64,
   ACC_MIN_F64, ACC_MAX_F64,   // stored as IEEE totalOrder keys so integer atomics apply
   ACC_MIN_DEC, ACC_MAX_DEC,   // 128-bit CAS loop
+  // FIRST / FIRST_IGNORES_NULL (first.rs, first_ignores_null.rs): the value of the eligible row with the smallest arrival
+  // ordinal.  `oword` holds that ordinal (identity ~0, "not set"); the value word(s) and the value's validity bit (`vbit`,
+  // 0xFF: never NULL) are written together with it under the slot lock.  Eligible rows:
+  ACC_FIRST,          // every row (nargs 1), or a row whose second argument (the merged `#flag` column) is non-zero (nargs 2)
+  ACC_FIRST_VALID,    // a row whose argument is valid
 };
+__host__ __device__ inline bool acc_is_first(uint8_t kind) { return kind == ACC_FIRST || kind == ACC_FIRST_VALID; }
 
 struct AccOp {
   uint8_t kind;
   uint8_t word;        // word offset inside the accumulator entry
   uint8_t vbit;        // bit in the slot header's flags marking "accumulator has a value" (0xFF: always valid)
-  uint8_t nargs;       // arguments (ACC_COUNT may have 0..4; others exactly 1)
+  uint8_t nargs;       // arguments (ACC_COUNT may have 0..4; others exactly 1, ACC_FIRST 1 or 2)
   uint8_t arg_out[4];  // VM output index of each argument
+  uint8_t oword;       // ACC_FIRST*: word of the arrival ordinal (ACC_FIRST accumulators of one aggregate share it)
+  uint8_t nwords;      // ACC_FIRST*: value words (2 for decimal128, else 1)
 };
 
 // The table is split in two arrays indexed by the slot number (tools/microbench/probes.cu compares the layouts: a probe
@@ -77,6 +85,8 @@ enum EmitKind : uint8_t {
   EMIT_ACC_VALUE,      // accumulator word(s) as a value of `phys` (valid iff its vbit is set / always)
   EMIT_AVG_F64,        // sum(word)/count(word2) -> f64            (avg.rs:166-171)
   EMIT_AVG_DEC,        // i128 sum div_euclid count -> decimal128   (avg.rs:158-165)
+  EMIT_FIRST_VALUE,    // FIRST value: valid iff the ordinal (word2) is set and the value's vbit is set (or vbit == 0xFF)
+  EMIT_FIRST_FLAG,     // FIRST `#flag` state column: int8 1 iff the ordinal (word2) is set
 };
 struct EmitCol {
   uint8_t kind, phys, word, word2;   // word: offset in the key entry (EMIT_KEY) or in the accumulator entry
@@ -91,9 +101,11 @@ constexpr int EMIT_MAX_COLS = 40;
 struct EmitTable { int32_t ncols; EmitCol col[EMIT_MAX_COLS]; };
 
 // frozen-row (reference Binary accumulator column) field descriptors
-enum FrozenKind : uint8_t { FZ_PRIM = 0, FZ_COUNT = 1 };
+// FZ_BOOL (AccBooleanColumn, acc.rs:180-207): one byte, 0 = NULL, else 1 + value.  With `valid` it is a Boolean value;
+// without, it is FIRST's flag over an int8 0/1 column (set: byte 2; any non-zero byte reads back as set)
+enum FrozenKind : uint8_t { FZ_PRIM = 0, FZ_COUNT = 1, FZ_BOOL = 2 };
 struct FrozenField {
-  uint8_t kind;        // FZ_PRIM: [u8 valid][LE value if valid] (acc.rs:335-346); FZ_COUNT: varint (count.rs:193-203)
+  uint8_t kind;        // FZ_PRIM: [u8 valid][LE value if valid] (acc.rs:335-346); FZ_COUNT: varint (count.rs:193-203); FZ_BOOL above
   uint8_t width;       // value bytes of FZ_PRIM (1,2,4,8,16)
   uint8_t phys;        // physical type of the state column
   uint8_t _pad;
@@ -120,11 +132,13 @@ int launch_filter_project_lean(const ColTable& cols, int ncols /*1..4, every one
                                void* d_work /* filter_project_lean_scratch_bytes(n) bytes, zeroed */, unsigned long long* d_scratch, cudaStream_t s);
 int64_t filter_project_lean_scratch_bytes(int64_t n);
 
+// ord_base: rows the op fed to the aggregate before this batch; row i of the batch has the arrival ordinal ord_base + i (FIRST)
 int launch_agg_update(const VmProgram* d_prog, const ColTable& cols, const AggLayout& lay, const AggTable& tab, int64_t row_begin, int64_t n,
-                      const uint32_t* d_row_list /*replay of deferred rows, or null*/, cudaStream_t s);
-// grouping sets: d_row_list entries (and the deferred entries it writes) are row * nsets + set; n counts rows, or list entries
+                      const uint32_t* d_row_list /*replay of deferred rows, or null*/, uint64_t ord_base, cudaStream_t s);
+// grouping sets: d_row_list entries (and the deferred entries it writes) are row * nsets + set; n counts rows, or list entries.
+// The arrival ordinal of (row, set) is (ord_base + row) * nsets + set
 int launch_agg_update_sets(const VmProgram* d_prog, const ColTable& cols, const AggLayout& lay, const AggTable& tab, int64_t row_begin, int64_t n,
-                           const uint32_t* d_row_list, const AggSetDesc* d_sets, int nsets, cudaStream_t s);
+                           const uint32_t* d_row_list, const AggSetDesc* d_sets, int nsets, uint64_t ord_base, cudaStream_t s);
 int launch_agg_rehash(const AggLayout& lay, const AggTable& old_tab, const AggTable& new_tab, cudaStream_t s);
 int launch_agg_emit(const AggLayout& lay, const AggTable& tab, const EmitTable& emit, unsigned long long* d_out_count, cudaStream_t s);
 int launch_pack_valid(const uint8_t* bytes, uint32_t* bits, int64_t n, cudaStream_t s);

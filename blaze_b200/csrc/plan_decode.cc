@@ -517,10 +517,18 @@ PlanP parse_agg(Reader r) {                  // AggExecNode (auron.proto:675-685
     if (!have_rt) bad("Missing required field in protobuf");
     if (modes[i] > 2) bad("invalid AggMode");
     a.mode = (AggMode)modes[i]; a.field_name = anames[i];
-    if (fn > 4) unsupported("aggregate function #" + std::to_string(fn) + " is out of the hot-path scope (variable-length / JVM-callback state)");
+    if (fn > 4 && fn != AGG_FIRST && fn != AGG_FIRST_IGNORES_NULL)
+      unsupported("aggregate function #" + std::to_string(fn) + " is out of the hot-path scope (variable-length / JVM-callback state)");
     a.fn = (AggFn)fn;
-    // create_agg (agg/agg.rs:171-205)
-    if (a.fn == AGG_COUNT) {
+    // create_agg (agg/agg.rs:171-213)
+    if (a.fn == AGG_FIRST || a.fn == AGG_FIRST_IGNORES_NULL) {
+      if (children.empty()) bad("aggregate without children");
+      // the child's type; a merge-side Placeholder has the Null type, so the state type comes from return_type
+      a.data_type = children[0]->type.id == T_NULL ? rt : children[0]->type;
+      if (a.data_type.is_varlen() || a.data_type.id == T_NULL)
+        unsupported(std::string(a.fn == AGG_FIRST ? "FIRST" : "FIRST_IGNORES_NULL") + " over " + a.data_type.str() + " is not on the hot path (fixed-width values only)");
+      a.args.push_back(children[0]);
+    } else if (a.fn == AGG_COUNT) {
       a.data_type = i64_t();
       for (auto& c : children) if (c->nullable) a.args.push_back(c);
     } else {
@@ -887,7 +895,8 @@ static void explain_rec(const PlanP& p, int depth, std::ostringstream& o) {
       for (size_t i = 0; i < p->proj_exprs.size(); i++) o << (i ? ", " : "") << explain_expr(p->proj_exprs[i]) << " AS " << p->schema.fields[i].name;
       o << "] schema=" << schema_str(p->schema) << "\n"; break;
     case N_AGG: {
-      static const char* fn[] = {"Min", "Max", "Sum", "Avg", "Count"}; static const char* md[] = {"Partial", "PartialMerge", "Final"};
+      static const char* fn[] = {"Min", "Max", "Sum", "Avg", "Count", "CollectList", "CollectSet", "First", "FirstIgnoresNull"};
+      static const char* md[] = {"Partial", "PartialMerge", "Final"};
       o << ind << "AggExec " << (p->exec_mode == 0 ? "HashAgg" : "SortAgg") << " groupings=[";
       for (size_t i = 0; i < p->group_exprs.size(); i++) o << (i ? ", " : "") << explain_expr(p->group_exprs[i]) << " AS " << p->group_names[i];
       o << "] aggs=[";

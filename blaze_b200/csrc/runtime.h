@@ -145,7 +145,7 @@ b200q_status fail(int code, const std::string& msg);
 b200q_status guarded_call(const std::function<void()>& f);        // exceptions -> status + b200q_last_error()
 
 // state columns of one aggregate in the columnar partial-state layout
-struct StateCols { std::vector<FieldDef> fields; };
+struct StateCols { std::vector<FieldDef> fields; std::vector<uint8_t> frozen; };   // frozen: FrozenKind of each field in the Binary agg-buffer column
 StateCols state_columns_of(const AggDef& a);
 
 }  // namespace b200q

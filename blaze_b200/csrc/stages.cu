@@ -299,13 +299,22 @@ static uint64_t host_mix64(uint64_t x) { x ^= x >> 33; x *= 0xff51afd7ed558ccdUL
 
 StateCols state_columns_of(const AggDef& a) {
   StateCols s; DType i64; i64.id = T_INT64;
+  const uint8_t value_kind = a.data_type.id == T_BOOL ? FZ_BOOL : FZ_PRIM;
   switch (a.fn) {
-    case AGG_COUNT: s.fields.push_back(FieldDef{a.field_name, i64, false}); break;
+    case AGG_COUNT: s.fields.push_back(FieldDef{a.field_name, i64, false}); s.frozen = {FZ_COUNT}; break;
     case AGG_AVG:
       s.fields.push_back(FieldDef{a.field_name + "#sum", a.data_type, true});
       s.fields.push_back(FieldDef{a.field_name + "#count", i64, false});
+      s.frozen = {FZ_PRIM, FZ_COUNT};
       break;
-    default: s.fields.push_back(FieldDef{a.field_name, a.data_type, true}); break;
+    case AGG_FIRST: {          // first.rs: the value, then the "set" flag (AccBooleanColumn); int8 in columnar form, as the exchange carries no Boolean
+      DType i8; i8.id = T_INT8;
+      s.fields.push_back(FieldDef{a.field_name, a.data_type, true});
+      s.fields.push_back(FieldDef{a.field_name + "#flag", i8, false});
+      s.frozen = {value_kind, FZ_BOOL};
+      break;
+    }
+    default: s.fields.push_back(FieldDef{a.field_name, a.data_type, true}); s.frozen = {value_kind}; break;
   }
   return s;
 }
@@ -400,6 +409,8 @@ class AggStage : public Stage {
   bool merge_mode_ = false, columnar_ = false, final_ = false;
   int n_in_ = 0;                        // input columns
   std::vector<FieldDef> merge_state_fields_;   // state columns fed by the merge-mode aggs (in agg order)
+  std::vector<uint8_t> merge_state_kinds_;     // their FrozenKind in the Binary agg-buffer column
+  uint64_t rows_pushed_ = 0;            // rows fed to the update before the current batch: the base of the FIRST arrival ordinals
   int first_state_col_ = 0;             // index of the first state column in the program's column space
   // grouping sets of a fused ExpandExec (nsets_ > 1): per-set keys and arguments over the shared VM outputs
   int nsets_ = 1;
@@ -424,7 +435,7 @@ class AggStage : public Stage {
   int64_t wide_rows_since_norm_ = 0;
 
   // emit plan (per output/state column)
-  struct EmitSpec { EmitCol ec; FieldDef field; bool frozen_count = false; };
+  struct EmitSpec { EmitCol ec; FieldDef field; bool frozen_count = false, frozen_bool = false; };
   std::vector<EmitSpec> emit_;          // key columns first, then per-agg result or state columns
   std::vector<FrozenField> frozen_fields_;     // non-final, reference format: how the state columns freeze
 
@@ -462,7 +473,11 @@ class AggStage : public Stage {
     }
 
     // ---- state columns consumed by merge-mode aggs
-    for (auto& a : agg.aggs) if (a.mode != MODE_PARTIAL) for (auto& f : state_columns_of(a).fields) merge_state_fields_.push_back(f);
+    for (auto& a : agg.aggs)
+      if (a.mode != MODE_PARTIAL) {
+        const StateCols sc = state_columns_of(a);
+        for (size_t k = 0; k < sc.fields.size(); k++) { merge_state_fields_.push_back(sc.fields[k]); merge_state_kinds_.push_back(sc.frozen[k]); }
+      }
     if (merge_mode_) {
       if (columnar_) {
         first_state_col_ = n_in_ - (int)merge_state_fields_.size();
@@ -522,6 +537,14 @@ class AggStage : public Stage {
       lay_.init[word] = init_lo; if (nwords == 2) lay_.init[word + 1] = init_hi;
       const int w = word; word += nwords; return w;
     };
+    // The FIRST accumulators of one aggregate take their values from the same row, so they share one ordinal word.  On the merge side the
+    // flags of one state row are equal for the same reason (the aggregate that wrote the state set them all from one row): the first
+    // FIRST's flag column decides for all of them, which keeps a wide dropDuplicates within AGG_MAX_ROW_WORDS
+    int first_oword[2] = {-1, -1}, first_flag_out = -1;     // [partial]: an op may mix update-side and merge-side aggregates
+    auto new_oword = [&]() {
+      if (word + 1 > AGG_MAX_SLOT_WORDS) throw PlanError(B200Q_ERR_UNSUPPORTED, "aggregate state too wide for one table slot");
+      lay_.init[word] = ~0ULL; return word++;
+    };
 
     // key emit columns
     for (int k = 0; k < lay_.nkeys; k++) {
@@ -536,6 +559,56 @@ class AggStage : public Stage {
       const DType& dt = a.data_type;
       if ((a.fn == AGG_MIN || a.fn == AGG_MAX) && dt.id == T_BOOL) throw PlanError(B200Q_ERR_UNSUPPORTED, "min/max over boolean is not on the hot path");
       int sum_word = -1, cnt_word = -1; uint8_t sum_vbit = 0xFF;
+      // --- First / FirstIgnoresNull: value word(s) + an arrival-ordinal word (kernels.cuh ACC_FIRST)
+      if (a.fn == AGG_FIRST || a.fn == AGG_FIRST_IGNORES_NULL) {
+        const bool ign = a.fn == AGG_FIRST_IGNORES_NULL;
+        const StateCols sc = state_columns_of(a);
+        std::vector<int> args;
+        bool value_nullable = true;
+        std::vector<int> set_o(nsets_, -1);
+        if (partial && !multi) { args.push_back(add_out(agg_args[ai][0])); value_nullable = can_be_null(agg_args[ai][0]); }
+        else if (partial) {                 // grouping sets: a NULL-literal value is AGG_NO_ARG in that set
+          value_nullable = false;
+          for (int s = 0; s < nsets_; s++) {
+            const ExprP& e = sets[s].agg_args[ai][0];
+            if (is_null_literal(e)) { value_nullable = true; continue; }
+            set_o[s] = add_out(e); value_nullable = value_nullable || can_be_null(e);
+          }
+          int o = 0; for (int s = nsets_ - 1; s >= 0; s--) if (set_o[s] >= 0) o = set_o[s];
+          args.push_back(o);
+        } else {
+          args.push_back(add_out(state_col_expr(sc.fields[0])));
+          if (!ign) {
+            const ExprP flag = state_col_expr(sc.fields[1]);
+            if (first_flag_out < 0) first_flag_out = add_out(flag);
+            args.push_back(first_flag_out);
+          }
+        }
+        // FirstIgnoresNull is valid iff set: only First needs a validity bit, and only for a value that can be NULL
+        const uint8_t vbit = (!ign && value_nullable) ? new_vbit() : (uint8_t)0xFF;
+        const int nwords = dt.is_decimal() ? 2 : 1;
+        const int vw = add_acc(ign ? ACC_FIRST_VALID : ACC_FIRST, nwords, vbit, args, 0, 0);
+        AccOp& op = lay_.acc[lay_.nacc - 1];
+        op.nwords = (uint8_t)nwords;
+        // FirstIgnoresNull follows its own value's validity: an ordinal word each
+        int ow;
+        if (!ign) { if (first_oword[partial] < 0) first_oword[partial] = new_oword(); ow = first_oword[partial]; }
+        else ow = new_oword();
+        op.oword = (uint8_t)ow;
+        for (int s = 0; multi && s < nsets_; s++) {
+          if (set_o[s] >= 0) sets_[s].acc_arg[lay_.nacc - 1][0] = (uint8_t)set_o[s];
+          else if (ign) sets_[s].acc_skip |= 1u << (lay_.nacc - 1);          // never a valid value in this set
+        }
+        auto first_spec = [&](const FieldDef& f, EmitKind kind) {
+          EmitSpec es{}; es.ec.kind = kind; es.ec.phys = phys_of(f.type); es.ec.word = (uint8_t)vw; es.ec.word2 = (uint8_t)ow; es.ec.vbit = vbit; es.field = f; return es;
+        };
+        if (final_) emit_.push_back(first_spec(agg.schema.fields[lay_.nkeys + ai], EMIT_FIRST_VALUE));
+        else {
+          emit_.push_back(first_spec(sc.fields[0], EMIT_FIRST_VALUE)); emit_.back().frozen_bool = sc.frozen[0] == FZ_BOOL;
+          if (!ign) { emit_.push_back(first_spec(sc.fields[1], EMIT_FIRST_FLAG)); emit_.back().frozen_bool = true; }
+        }
+        continue;
+      }
       // --- sum-like part (Sum, Avg, Min, Max)
       if (a.fn != AGG_COUNT) {
         ExprP arg;
@@ -669,7 +742,7 @@ class AggStage : public Stage {
     if (!final_) {
       for (size_t i = lay_.nkeys; i < emit_.size(); i++) {
         FrozenField f{}; const FieldDef& fd = emit_[i].field;
-        f.kind = emit_[i].frozen_count ? FZ_COUNT : FZ_PRIM; f.width = frozen_width(fd.type); f.phys = phys_of(fd.type);
+        f.kind = emit_[i].frozen_count ? FZ_COUNT : emit_[i].frozen_bool ? FZ_BOOL : FZ_PRIM; f.width = frozen_width(fd.type); f.phys = phys_of(fd.type);
         frozen_fields_.push_back(f);
       }
     }
@@ -693,6 +766,8 @@ class AggStage : public Stage {
     return -1;
   }
   static bool int_phys(const DType& t) { return t.is_intlike(); }
+  // FIRST needs the arrival ordinal of every row: only the generic (VM) update kernels carry it
+  bool has_first() const { for (int j = 0; j < lay_.nacc; j++) if (acc_is_first(lay_.acc[j].kind)) return true; return false; }
 
   // the 1-2 integer key columns and the `col cmp literal` conjuncts of the specialised kernels (key slots, filt[], merged
   // into frange[] by merge_conjuncts); false: a key or a conjunct they cannot read
@@ -721,7 +796,7 @@ class AggStage : public Stage {
 
   void detect_fast(OpContext& cx) {
     fast_ok_ = false;
-    if (cx.conf.force_generic_kernels) return;
+    if (cx.conf.force_generic_kernels || has_first()) return;
     if (lay_.nacc < 1 || lay_.nacc > 2) return;
     FastSpec fs{};
     if (!parse_keys_and_conjuncts(fs)) return;
@@ -794,7 +869,7 @@ class AggStage : public Stage {
   // (a decimal128 argument takes both value registers).  Dense keys only (decided on the first batch like DENSE mode).
   void detect_wide(OpContext& cx) {
     wide_possible_ = false;
-    if (cx.conf.force_generic_kernels || !cx.conf.agg_dense_keys) return;
+    if (cx.conf.force_generic_kernels || !cx.conf.agg_dense_keys || has_first()) return;
     if (lay_.nacc < 1 || lay_.nacc > 4) return;
     TileAggSpec ts{};
     {
@@ -1031,7 +1106,7 @@ class AggStage : public Stage {
   }
 
   int launch_update(OpContext& cx, const ColTable& ct, const AggTable& t, int64_t begin, int64_t m, const uint32_t* list) {
-    if (nsets_ > 1) return launch_agg_update_sets((const VmProgram*)d_prog_->ptr, ct, lay_, t, begin, m, list, (const AggSetDesc*)d_sets_->ptr, nsets_, cx.stream);
+    if (nsets_ > 1) return launch_agg_update_sets((const VmProgram*)d_prog_->ptr, ct, lay_, t, begin, m, list, (const AggSetDesc*)d_sets_->ptr, nsets_, rows_pushed_, cx.stream);
     // deferred-row replays (arbitrary row lists, rare) always take the generic kernel: same table, same semantics
     if (wide_possible_ && ws_.dense_tab && !list) {
       cx.m.fast_launches++;
@@ -1047,7 +1122,7 @@ class AggStage : public Stage {
       fs.lean = lean_ok(ct, begin) ? 1 : 0;
       return launch_agg_fast_update(ct, fs, lay_, t, begin, m, cx.stream);
     }
-    return launch_agg_update((const VmProgram*)d_prog_->ptr, ct, lay_, t, begin, m, list, cx.stream);
+    return launch_agg_update((const VmProgram*)d_prog_->ptr, ct, lay_, t, begin, m, list, rows_pushed_, cx.stream);
   }
 
   // A12: the GPU table never spills; when it would outgrow its HBM budget (b200q_conf.agg_max_table_bytes, or the
@@ -1229,6 +1304,7 @@ class AggStage : public Stage {
     }
     if (!dense_decided_) { if (wide_possible_) decide_wide(cx, ct, n); else decide_dense(cx, ct, n); }
     update_rows(cx, ct, n);
+    rows_pushed_ += (uint64_t)n;
   }
 
   // Binary agg-buffer column -> typed state columns (AccColumn::unfreeze_from_rows, agg_ctx.rs:276-296)
@@ -1239,18 +1315,23 @@ class AggStage : public Stage {
     FrozenTable ft{}; ft.nfields = (int)merge_state_fields_.size();
     if (ft.nfields > FROZEN_MAX_FIELDS) throw ExecError(B200Q_ERR_UNSUPPORTED, "too many accumulator fields");
     std::vector<DevMemP> valid_bytes(ft.nfields);
+    std::vector<DevMemP> bool_bytes(ft.nfields);
     for (int k = 0; k < ft.nfields; k++) {
       const FieldDef& f = merge_state_fields_[k];
-      DevColumn c; c.type = f.type; c.values = DevMem::alloc((size_t)n * f.type.byte_width(), cx.stream);
+      DevColumn c; c.type = f.type;
       FrozenField& ff = ft.f[k];
-      ff.kind = f.nullable ? FZ_PRIM : FZ_COUNT; ff.width = frozen_width(f.type); ff.phys = phys_of(f.type); ff.values = c.values->ptr;
+      ff.kind = merge_state_kinds_[k]; ff.width = frozen_width(f.type); ff.phys = phys_of(f.type);
+      if (f.type.id == T_BOOL) { bool_bytes[k] = DevMem::alloc((size_t)n, cx.stream); ff.values = bool_bytes[k]->ptr; c.values = DevMem::alloc(bitmap_bytes(n), cx.stream); }
+      else { c.values = DevMem::alloc((size_t)n * f.type.byte_width(), cx.stream); ff.values = c.values->ptr; }
       if (f.nullable) { valid_bytes[k] = DevMem::alloc((size_t)n, cx.stream); ff.valid = (const uint8_t*)valid_bytes[k]->ptr; c.validity = DevMem::alloc(bitmap_bytes(n), cx.stream); }
       state_cols.push_back(c);
     }
     int* d_err = (int*)((unsigned long long*)counters_->ptr + 2);
     cx.m.launches += launch_frozen_read(ft, n, (const int32_t*)bc.offsets->ptr, bc.offset, (const uint8_t*)bc.values->ptr, d_err, cx.stream);
-    for (int k = 0; k < ft.nfields; k++)
+    for (int k = 0; k < ft.nfields; k++) {
       if (valid_bytes[k]) cx.m.launches += launch_pack_valid((const uint8_t*)valid_bytes[k]->ptr, (uint32_t*)state_cols[k].validity->ptr, n, cx.stream);
+      if (bool_bytes[k]) cx.m.launches += launch_pack_valid((const uint8_t*)bool_bytes[k]->ptr, (uint32_t*)state_cols[k].values->ptr, n, cx.stream);
+    }
     B200Q_CUDA(cudaGetLastError());
     // valid_bytes buffers are released stream-ordered after the pack kernels
   }
@@ -1301,7 +1382,7 @@ class AggStage : public Stage {
       FrozenTable ft{}; ft.nfields = (int)frozen_fields_.size();
       for (int k = 0; k < ft.nfields; k++) {
         ft.f[k] = frozen_fields_[k];
-        ft.f[k].values = ob.cols[lay_.nkeys + k].values->ptr;
+        ft.f[k].values = bool_bytes[lay_.nkeys + k] ? bool_bytes[lay_.nkeys + k]->ptr : ob.cols[lay_.nkeys + k].values->ptr;   // Boolean: one byte per row
         ft.f[k].valid = valid_bytes[lay_.nkeys + k] ? (const uint8_t*)valid_bytes[lay_.nkeys + k]->ptr : nullptr;
       }
       DevMemP lengths = DevMem::alloc((size_t)g * 4, cx.stream);

@@ -287,7 +287,9 @@ class ScalarFunction(Expr):
 
 # AggFunction enum values (auron.proto:127-141)
 AGG_MIN, AGG_MAX, AGG_SUM, AGG_AVG, AGG_COUNT = 0, 1, 2, 3, 4
-AGG_NAMES = {AGG_MIN: "Min", AGG_MAX: "Max", AGG_SUM: "Sum", AGG_AVG: "Avg", AGG_COUNT: "Count"}
+AGG_FIRST, AGG_FIRST_IGNORES_NULL = 7, 8
+AGG_NAMES = {AGG_MIN: "Min", AGG_MAX: "Max", AGG_SUM: "Sum", AGG_AVG: "Avg", AGG_COUNT: "Count",
+             AGG_FIRST: "First", AGG_FIRST_IGNORES_NULL: "FirstIgnoresNull"}
 
 # AggMode (auron.proto:692-696) / AggExecMode (:687-690)
 PARTIAL, PARTIAL_MERGE, FINAL = 0, 1, 2

@@ -398,7 +398,10 @@ def _agg_data_type(f: AggFunctionExpr, ins: Schema) -> T.DataType:
         return T.int64
     if f.function in (E.AGG_SUM, E.AGG_AVG):
         return f.return_type
-    return f.children[0].data_type(ins)
+    dt = f.children[0].data_type(ins)
+    if f.function in (E.AGG_FIRST, E.AGG_FIRST_IGNORES_NULL) and dt == T.null:
+        return f.return_type                                                                          # merge side: Placeholder of type Null
+    return dt
 
 
 def _agg_final_type(f: AggFunctionExpr, ins: Schema) -> T.DataType:
@@ -414,4 +417,6 @@ def _state_fields(a: AggExpr, ins: Schema) -> List[Field]:
         return [Field(a.field_name, T.int64, False)]
     if a.agg.function == E.AGG_AVG:
         return [Field(a.field_name + "#sum", dt, True), Field(a.field_name + "#count", T.int64, False)]
+    if a.agg.function == E.AGG_FIRST:                                                                # value, then the "set" flag as int8 0/1
+        return [Field(a.field_name, dt, True), Field(a.field_name + "#flag", T.int8, False)]
     return [Field(a.field_name, dt, True)]

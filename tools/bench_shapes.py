@@ -541,3 +541,80 @@ if any(t in (ONLY or "W1,W2") for t in ("W1", "W2")):
         expect = int(((head - pstart + 1) <= 100).sum())
         print(json.dumps({"shape": "W2 SortExec(p, o) -> WindowExec(rank, group limit 100)", "rows": n2, "out_rows": n_out, "verified": n_out == expect,
                           "wall_ms_push_to_sync": dt * 1e3, "rows_per_s": n2 / dt, "launches": m["gpu_kernel_launches"]}), flush=True)
+
+
+# F1-F2: FIRST in AggExec over 2^26 device-resident rows, whole-op wall time push_device -> finish -> sync, Partial and Final fused in one op.
+# F1 is Dataset.dropDuplicates(k): k ~ U[0, 2^20), FIRST(ignoreNulls = false) over four int64 columns; 40 algorithmic bytes per row.
+# F2 is SUM(v), FIRST_IGNORES_NULL(w) GROUP BY k (k ~ U[0, 2^20), w 30% NULL) next to SUM(v) GROUP BY k on its own kernel and on the
+# generic VM kernel (force_generic_kernels), alternated in one call: a FIRST accumulator takes the aggregate off the lean kernel onto the
+# VM kernel, and the three figures split that cost into leaving the lean kernel and the FIRST accumulator itself.
+def run_first_wall(name, plan, spec, keep, n, alg_bytes, conf=None):
+    if ONLY and not any(t in name for t in ONLY.split(",")): return
+    import time
+    best = None
+    for _ in range(REPS or 5):
+        with native.NativeOp(plan.plan_bytes(), conf or native.default_conf(), 0) as op:
+            torch.cuda.synchronize(); t0 = time.perf_counter()
+            op.push_device(native.DeviceBatch(spec, n, 0, keepalive=keep))
+            op.finish(); op.sync()
+            dt = time.perf_counter() - t0
+            m = op.metrics(); n_out = 0
+            while True:
+                o = op.pull_device()
+                if o is None: break
+                n_out += o.array.length; native.release_device_array(o)
+        if best is None or dt < best[0]: best = (dt, m, n_out)
+    return best
+
+
+if any(t in (ONLY or "F1,F2") for t in ("F1", "F2")):
+    import subprocess
+    card = torch.cuda.get_device_name(0)
+    try:
+        plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True).stdout.strip()
+    except OSError:
+        plim = "unknown"
+    frows = int(os.environ.get("ROWS", 1 << 26))
+    fk = torch.randint(0, 1 << 20, (frows,), dtype=torch.int64, device=dev, generator=g)
+    n_keys = int(torch.unique(fk).numel())
+    fc = [torch.randint(-2**62, 2**62, (frows,), dtype=torch.int64, device=dev, generator=g) for _ in range(4)]
+    f_sch = T.Schema([T.Field("k", T.int64, False)] + [T.Field(f"c{i}", T.int64, False) for i in range(4)])
+    f_g = [E.GroupingExpr("k", E.Column("k"))]
+    f_aggs = lambda mode: [E.AggExpr(f"c{i}", mode, PL.create_agg(E.AGG_FIRST, [E.Column(f"c{i}") if mode == E.PARTIAL else E.placeholder()], f_sch, T.int64))
+                           for i in range(4)]
+    f1 = PL.AggExec(PL.HashAgg, f_g, f_aggs(E.FINAL), False, PL.AggExec(PL.HashAgg, f_g, f_aggs(E.PARTIAL), False, PL.MemoryExec(f_sch)))
+    r = run_first_wall("F1", f1, [(t.data_ptr(), 0, frows) for t in [fk] + fc], [fk] + fc, frows, 40.0)
+    if r:
+        dt, m, n_out = r
+        print(json.dumps({"shape": "F1 dropDuplicates(k): FIRST over four int64 columns, 2^20 keys", "card": card, "power_limit": plim, "rows": frows,
+                          "out_rows": n_out, "verified_groups": n_out == n_keys, "wall_ms_push_to_sync": dt * 1e3, "rows_per_s": frows / dt,
+                          "alg_GBps": 40.0 * frows / dt / 1e9, "frac_of_hbm_peak": 40.0 * frows / dt / 1e9 / peak, "fast_path_launches": m["fast_path_launches"],
+                          "launches": m["gpu_kernel_launches"]}), flush=True)
+    del fc
+    fv = torch.randint(-10**6, 10**6, (frows,), dtype=torch.int64, device=dev, generator=g)
+    fw = torch.randint(-10**6, 10**6, (frows,), dtype=torch.int64, device=dev, generator=g)
+    fwv = torch.rand(frows, device=dev, generator=g) >= 0.3
+    fw_valid = torch.from_numpy(__import__("numpy").packbits(fwv.cpu().numpy(), bitorder="little")).to(dev)
+    s2 = T.Schema([T.Field("k", T.int64, False), T.Field("v", T.int64, False), T.Field("w", T.int64, True)])
+    def f2_plan(with_first):
+        def a(mode):
+            out = [E.AggExpr("s", mode, PL.create_agg(E.AGG_SUM, [E.Column("v") if mode == E.PARTIAL else E.placeholder(T.int64)], s2, T.int64))]
+            if with_first:
+                out.append(E.AggExpr("w", mode, PL.create_agg(E.AGG_FIRST_IGNORES_NULL, [E.Column("w") if mode == E.PARTIAL else E.placeholder()], s2, T.int64)))
+            return out
+        return PL.AggExec(PL.HashAgg, f_g, a(E.FINAL), False, PL.AggExec(PL.HashAgg, f_g, a(E.PARTIAL), False, PL.MemoryExec(s2)))
+    spec2 = [(fk.data_ptr(), 0, frows), (fv.data_ptr(), 0, frows), (fw.data_ptr(), fw_valid.data_ptr(), frows)]
+    variants = {"F2 SUM(v), FIRST_IGNORES_NULL(w) GROUP BY k": (True, None), "F2-base SUM(v) GROUP BY k (same call)": (False, None),
+                "F2-generic SUM(v) GROUP BY k on the VM kernel (same call)": (False, native.default_conf(force_generic_kernels=1))}
+    res = {v: [] for v in variants}
+    for _ in range(3):                                   # alternate the plans in this call
+        for v, (wf, cf) in variants.items():
+            r = run_first_wall("F2", f2_plan(wf), spec2, [fk, fv, fw, fw_valid], frows, 24.0, cf)
+            if r: res[v].append(r)
+    if all(res.values()):
+        for v in variants:
+            dt, m, n_out = min(res[v], key=lambda x: x[0])
+            print(json.dumps({"shape": v, "card": card,
+                              "power_limit": plim, "rows": frows, "out_rows": n_out, "verified_groups": n_out == n_keys, "wall_ms_push_to_sync": dt * 1e3,
+                              "rows_per_s": frows / dt, "wall_ms_all_runs": [round(x[0] * 1e3, 2) for x in res[v]], "fast_path_launches": m["fast_path_launches"],
+                              "launches": m["gpu_kernel_launches"]}), flush=True)
