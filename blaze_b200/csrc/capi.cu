@@ -99,6 +99,7 @@ struct b200q_op {
   StagingSet staging[2]; int cur_stage_set = 0; bool staging_ready = false;
   cudaEvent_t ev_a = nullptr, ev_b = nullptr;
   std::shared_ptr<StreamRef> stream_ref;
+  std::unique_ptr<IpcSource> ipc;   // the op's source when its leaf is an IpcReaderExecNode (input through b200q_op_push_ipc only)
 };
 
 namespace b200q {
@@ -657,6 +658,9 @@ b200q_status b200q_op_create(const uint8_t* plan, size_t plan_len, int32_t plan_
     op->cx.stream = op->stream_ref->s;
     B200Q_CUDA(cudaEventCreate(&op->cx.ev0)); B200Q_CUDA(cudaEventCreate(&op->cx.ev1));
     build_pipeline(op);
+    const PlanNode* leaf = op->plan.get();
+    while (leaf->input) leaf = leaf->input.get();
+    if (leaf->leaf_kind == "IpcReader") op->ipc = make_ipc_source(op->cx, op->in_schema, op->stages[0]->used_input_cols);
     if (input_schema) {
       if (input_schema->n_children != (int64_t)op->in_schema.fields.size()) throw PlanError(B200Q_ERR_INVALID_ARG, "input_schema does not match the plan leaf: column count");
       for (int64_t i = 0; i < input_schema->n_children; i++)
@@ -682,6 +686,7 @@ b200q_status b200q_op_push(b200q_op* op, struct ArrowArray* batch) {
   if (!op) return fail(B200Q_ERR_INVALID_ARG, "op is null");
   b200q_status st = guarded(op, [&] {
     if (op->finished) throw ExecError(B200Q_ERR_STATE, "push after finish");
+    if (op->ipc) throw ExecError(B200Q_ERR_STATE, "an op whose leaf is an IpcReaderExecNode takes its input through b200q_op_push_ipc");
     B200Q_CUDA(cudaSetDevice(op->cx.device));
     validate_host_batch(op, batch);
     poll_pending(op, false);
@@ -703,10 +708,23 @@ b200q_status b200q_op_push(b200q_op* op, struct ArrowArray* batch) {
   return st;
 }
 
+b200q_status b200q_op_push_ipc(b200q_op* op, const uint8_t* data, size_t len) {
+  if (!op) return fail(B200Q_ERR_INVALID_ARG, "op is null");
+  return guarded(op, [&] {
+    if (op->finished) throw ExecError(B200Q_ERR_STATE, "push after finish");
+    if (!op->ipc) throw ExecError(B200Q_ERR_STATE, "push_ipc: the op's leaf is not an IpcReaderExecNode");
+    if (!data && len) throw ExecError(B200Q_ERR_INVALID_ARG, "push_ipc: null data");
+    B200Q_CUDA(cudaSetDevice(op->cx.device));
+    poll_pending(op, false);
+    op->ipc->push(op->cx, data, len, [&](DevBatch& b) { run_stages(op, b, 0); });
+  });
+}
+
 b200q_status b200q_op_push_device(b200q_op* op, struct ArrowDeviceArray* dbatch) {
   if (!op) return fail(B200Q_ERR_INVALID_ARG, "op is null");
   b200q_status st = guarded(op, [&] {
     if (op->finished) throw ExecError(B200Q_ERR_STATE, "push after finish");
+    if (op->ipc) throw ExecError(B200Q_ERR_STATE, "an op whose leaf is an IpcReaderExecNode takes its input through b200q_op_push_ipc");
     if (!dbatch) throw ExecError(B200Q_ERR_INVALID_ARG, "null batch");
     if (dbatch->device_type != ARROW_DEVICE_CUDA || dbatch->device_id != op->cx.device) throw ExecError(B200Q_ERR_INVALID_ARG, "push_device: batch is not on this op's CUDA device");
     B200Q_CUDA(cudaSetDevice(op->cx.device));
@@ -753,6 +771,7 @@ b200q_status b200q_op_finish(b200q_op* op) {
         run_parquet_scan(op->cx, *leaf, [&](DevBatch& b) { run_stages(op, b, 0); });
       }
     }
+    if (op->ipc) op->ipc->flush(op->cx, [&](DevBatch& b) { run_stages(op, b, 0); });
     if (op->staging_ready) staging_flush(op);
     for (size_t i = 0; i < op->stages.size(); i++) {
       std::vector<DevBatch> outs;
@@ -829,6 +848,7 @@ void b200q_op_destroy(b200q_op* op) {
   if (op->cx.stream) cudaStreamSynchronize(op->cx.stream);
   poll_pending(op, true);
   op->out_queue.clear(); op->has_cur_host = false; op->cur_host = HostBatch();
+  op->ipc.reset();
   op->stages.clear();
   staging_free(op);
   if (op->cx.ev0) cudaEventDestroy(op->cx.ev0);
@@ -902,6 +922,23 @@ b200q_status b200q_lz4_frame_compress(const uint8_t* src, size_t n, uint8_t* dst
     *out_len = v.size();
     if (!dst || cap < v.size()) throw ExecError(B200Q_ERR_INVALID_ARG, "lz4 frame needs " + std::to_string(v.size()) + " bytes");
     memcpy(dst, v.data(), v.size());
+  });
+}
+
+b200q_status b200q_lz4_frame_decompress(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, size_t* out_len) {
+  if ((!src && n) || !out_len) return fail(B200Q_ERR_INVALID_ARG, "null argument");
+  return guarded(nullptr, [&] {
+    size_t bound = 0;
+    try {
+      bound = lz4_frame_bound(src, n);
+      if (dst && cap >= bound) { *out_len = lz4_frame_decompress(src, n, dst, cap); return; }
+      std::vector<uint8_t> v(bound);                  // the exact size is known only once decoded
+      *out_len = lz4_frame_decompress(src, n, v.data(), v.size());
+      if (dst && cap >= *out_len) { memcpy(dst, v.data(), *out_len); return; }
+    } catch (const Lz4FrameError& e) {
+      throw ExecError(B200Q_ERR_INVALID_ARG, std::string(e.what()) + " at byte " + std::to_string(e.offset));
+    }
+    throw ExecError(B200Q_ERR_INVALID_ARG, "lz4 frame content needs " + std::to_string(*out_len) + " bytes");
   });
 }
 

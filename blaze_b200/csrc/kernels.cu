@@ -978,10 +978,26 @@ __device__ __forceinline__ V16 shifted16(const V16* __restrict__ src, int v, uns
   return r;
 }
 
+// n bytes sp -> dp by the whole warp.  Runs of 64 bytes or more are stored as aligned 16-byte vectors: the loads are aligned
+// 16-byte vectors too, shifted into place when source and destination disagree modulo 16 (both loads of a lane hold at least one
+// byte of the run, so they stay inside its buffer).  Heads and tails are coalesced byte copies.
+__device__ __forceinline__ void warp_copy_bytes(const uint8_t* sp, uint8_t* dp, int n, unsigned lane) {
+  int done = 0;
+  if (n >= 64) {
+    const int head = (int)((16 - ((uintptr_t)dp & 15)) & 15);
+    if ((int)lane < head) dp[lane] = sp[lane];
+    const int nv = (n - head) >> 4;
+    const uint8_t* s = sp + head; V16* vd = (V16*)(dp + head);
+    const unsigned mis = (unsigned)((uintptr_t)s & 15);
+    if (mis == 0) { const V16* vs = (const V16*)s; for (int v = (int)lane; v < nv; v += 32) vd[v] = vs[v]; }
+    else { const V16* vs = (const V16*)(s - mis); for (int v = (int)lane; v < nv; v += 32) vd[v] = shifted16(vs, v, mis); }
+    done = head + (nv << 4);
+  }
+  for (int b = done + (int)lane; b < n; b += 32) dp[b] = sp[b];
+}
+
 // One warp per group of 32 output rows; the rows are copied one after the other by the whole warp, so a long string spreads over
-// 32 lanes (and every warp of the grid keeps its own rows).  Strings of 64 bytes or more are stored as aligned 16-byte vectors: the
-// loads are aligned 16-byte vectors too, shifted into place when source and destination disagree modulo 16 (both loads of a lane hold
-// at least one byte of the string, so they stay inside its buffer).  Heads and tails are coalesced byte copies.
+// 32 lanes (and every warp of the grid keeps its own rows).
 __global__ void __launch_bounds__(256) varlen_copy_kernel(const DevCol src, const uint32_t* __restrict__ sel, long long m,
                                                           const int32_t* __restrict__ out_offsets, uint8_t* __restrict__ out) {
   const unsigned lane = threadIdx.x & 31;
@@ -992,23 +1008,8 @@ __global__ void __launch_bounds__(256) varlen_copy_kernel(const DevCol src, cons
     long long s0 = 0, d0 = 0; int len = 0;
     if (i < m) { const long long j = sel ? (long long)sel[i] : i; s0 = src.offsets[j]; len = src.offsets[j + 1] - (int32_t)s0; d0 = out_offsets[i]; }
     const int cnt = (int)(m - base < 32 ? m - base : 32);
-    for (int k = 0; k < cnt; k++) {
-      const uint8_t* sp = data + __shfl_sync(0xffffffffu, s0, k);
-      uint8_t* dp = out + __shfl_sync(0xffffffffu, d0, k);
-      const int n = __shfl_sync(0xffffffffu, len, k);
-      int done = 0;
-      if (n >= 64) {
-        const int head = (int)((16 - ((uintptr_t)dp & 15)) & 15);
-        if ((int)lane < head) dp[lane] = sp[lane];
-        const int nv = (n - head) >> 4;
-        const uint8_t* s = sp + head; V16* vd = (V16*)(dp + head);
-        const unsigned mis = (unsigned)((uintptr_t)s & 15);
-        if (mis == 0) { const V16* vs = (const V16*)s; for (int v = (int)lane; v < nv; v += 32) vd[v] = vs[v]; }
-        else { const V16* vs = (const V16*)(s - mis); for (int v = (int)lane; v < nv; v += 32) vd[v] = shifted16(vs, v, mis); }
-        done = head + (nv << 4);
-      }
-      for (int b = done + (int)lane; b < n; b += 32) dp[b] = sp[b];
-    }
+    for (int k = 0; k < cnt; k++)
+      warp_copy_bytes(data + __shfl_sync(0xffffffffu, s0, k), out + __shfl_sync(0xffffffffu, d0, k), __shfl_sync(0xffffffffu, len, k), lane);
   }
 }
 
@@ -1020,6 +1021,111 @@ int launch_varlen_lengths(const DevCol& src, const uint32_t* sel, int64_t m, int
 int launch_varlen_copy(const DevCol& src, const uint32_t* sel, int64_t m, const int32_t* out_offsets, uint8_t* out_data, cudaStream_t s) {
   if (m <= 0) return 0;
   varlen_copy_kernel<<<grid_for((m + 255) / 256, 8), 256, 0, s>>>(src, sel, m, out_offsets, out_data);
+  return 1;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// IpcReaderExec: batch_serde records -> coalesced columns (the inverse of the shuffle encode kernels).  Every extent a kernel
+// reads was checked by the host walk of the records (ipc_records.cc) before the launch.
+// ---------------------------------------------------------------------------------------------------
+// `W` byte planes of `rows` bytes -> `rows` little-endian values of W bytes.  A warp reads 32 consecutive bytes of each plane
+// (one sector per plane) and stores 32 whole values: one naturally aligned store per value (16 bytes for decimal128).
+template <int W>
+__device__ __forceinline__ void ipc_untranspose(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, long long rows, long long r0, long long r1) {
+  for (long long r = r0 + threadIdx.x; r < r1; r += blockDim.x) {
+    unsigned long long lo = 0, hi = 0;
+#pragma unroll
+    for (int k = 0; k < W; k++) {
+      const unsigned long long b = __ldg(src + (long long)k * rows + r);
+      if (k < 8) lo |= b << (8 * k); else hi |= b << (8 * (k - 8));
+    }
+    if constexpr (W == 16) { V16 v; v.lo = lo; v.hi = hi; ((V16*)dst)[r] = v; }
+    else if constexpr (W == 8) ((unsigned long long*)dst)[r] = lo;
+    else if constexpr (W == 4) ((uint32_t*)dst)[r] = (uint32_t)lo;
+    else if constexpr (W == 2) ((uint16_t*)dst)[r] = (uint16_t)lo;
+    else dst[r] = (uint8_t)lo;
+  }
+}
+
+// one block per (record, column) tile of IPC_TILE rows; one launch covers every fixed-width column of a flush
+__global__ void __launch_bounds__(256) ipc_decode_fixed_kernel(const IpcFixedJob* __restrict__ jobs, const IpcTile* __restrict__ tiles, long long ntiles) {
+  for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    const IpcTile tl = tiles[t];
+    const IpcFixedJob j = jobs[tl.job];
+    const long long r0 = (long long)tl.row0, r1 = r0 + IPC_TILE < j.rows ? r0 + IPC_TILE : j.rows;
+    switch (j.width) {
+      case 1: ipc_untranspose<1>(j.src, j.dst, j.rows, r0, r1); break;
+      case 2: ipc_untranspose<2>(j.src, j.dst, j.rows, r0, r1); break;
+      case 4: ipc_untranspose<4>(j.src, j.dst, j.rows, r0, r1); break;
+      case 8: ipc_untranspose<8>(j.src, j.dst, j.rows, r0, r1); break;
+      default: ipc_untranspose<16>(j.src, j.dst, j.rows, r0, r1); break;
+    }
+  }
+}
+
+// Validity bitmaps and Boolean values: records start at any output row, so their bits are re-packed at a bit offset.  One thread
+// per output word (no atomics): it finds the record holding the word's first row and takes up to 32 bits from each record the
+// word overlaps, as a funnel shift of the (at most 5) source bytes that hold them.  A record without a bitmap (src null) gives
+// all-valid bits.
+__global__ void __launch_bounds__(256) ipc_decode_bits_kernel(const IpcBitCol* __restrict__ cols, int ncols, const long long* __restrict__ rec_row, long long nrec, long long rows) {
+  const long long nwords = (rows + 31) >> 5;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < nwords * ncols; t += (long long)gridDim.x * blockDim.x) {
+    const IpcBitCol c = cols[t / nwords];
+    const long long w = t % nwords;
+    const long long b0 = w << 5, b1 = b0 + 32 < rows ? b0 + 32 : rows;
+    long long lo = 0, hi = nrec - 1;                                   // the last record that starts at or before b0
+    while (lo < hi) { const long long mid = (lo + hi + 1) >> 1; if (rec_row[mid] <= b0) lo = mid; else hi = mid - 1; }
+    uint32_t word = 0;
+    for (long long r = lo, b = b0; b < b1; r++) {
+      const long long rs = rec_row[r], rn = rec_row[r + 1], re = rn < b1 ? rn : b1;
+      if (re <= b) continue;                                           // a record of 0 rows
+      const int len = (int)(re - b);
+      const uint32_t mask = len == 32 ? 0xFFFFFFFFu : (1u << len) - 1;
+      const uint8_t* src = c.src[r];
+      uint32_t bits = mask;
+      if (src) {
+        const long long sb = b - rs, byte = sb >> 3, nbytes = (rn - rs + 7) >> 3;
+        unsigned long long v = 0;
+#pragma unroll
+        for (int k = 0; k < 5; k++) if (byte + k < nbytes) v |= (unsigned long long)__ldg(src + byte + k) << (8 * k);
+        bits = (uint32_t)(v >> (sb & 7)) & mask;
+      }
+      word |= bits << (int)(b - b0);
+      b = re;
+    }
+    c.dst[w] = word;
+  }
+}
+
+// Binary / Utf8 row bytes: each record's bytes are contiguous in the stream and in the output, so a flush is a list of range
+// copies (cut by the host into pieces of at most IPC_COPY_PIECE bytes).  Each warp loads 32 pieces (one per lane) and copies them one
+// after the other, as varlen_copy_kernel does with rows.
+__global__ void __launch_bounds__(256) ipc_decode_bytes_kernel(const IpcCopy* __restrict__ copies, long long n) {
+  const unsigned lane = threadIdx.x & 31;
+  const long long warps = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long base = ((blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5) * 32; base < n; base += warps * 32) {
+    const long long i = base + lane;
+    unsigned long long sp = 0, dp = 0; int len = 0;
+    if (i < n) { sp = (unsigned long long)copies[i].src; dp = (unsigned long long)copies[i].dst; len = (int)copies[i].len; }
+    const int cnt = (int)(n - base < 32 ? n - base : 32);
+    for (int k = 0; k < cnt; k++)
+      warp_copy_bytes((const uint8_t*)__shfl_sync(0xffffffffu, sp, k), (uint8_t*)__shfl_sync(0xffffffffu, dp, k), __shfl_sync(0xffffffffu, len, k), lane);
+  }
+}
+
+int launch_ipc_decode_fixed(const IpcFixedJob* jobs, const IpcTile* tiles, int64_t ntiles, cudaStream_t s) {
+  if (ntiles <= 0) return 0;
+  ipc_decode_fixed_kernel<<<grid_for(ntiles, 8), 256, 0, s>>>(jobs, tiles, ntiles);
+  return 1;
+}
+int launch_ipc_decode_bits(const IpcBitCol* cols, int ncols, const int64_t* rec_row, int64_t nrec, int64_t rows, cudaStream_t s) {
+  if (ncols <= 0 || rows <= 0) return 0;
+  ipc_decode_bits_kernel<<<grid_for(((rows + 31) / 32 * ncols + 255) / 256, 8), 256, 0, s>>>(cols, ncols, (const long long*)rec_row, nrec, rows);
+  return 1;
+}
+int launch_ipc_decode_bytes(const IpcCopy* copies, int64_t n, cudaStream_t s) {
+  if (n <= 0) return 0;
+  ipc_decode_bytes_kernel<<<grid_for((n + 7) / 8, 8), 256, 0, s>>>(copies, n);
   return 1;
 }
 

@@ -155,4 +155,15 @@ int64_t scan_num_blocks(int64_t n);
 int launch_varlen_lengths(const DevCol& src, const uint32_t* sel, int64_t m, int32_t* lengths, uint32_t* out_valid, unsigned long long* d_total, cudaStream_t s);
 int launch_varlen_copy(const DevCol& src, const uint32_t* sel, int64_t m, const int32_t* out_offsets, uint8_t* out_data, cudaStream_t s);
 
+// IpcReaderExec decode (ipc_source.cu drives them): batch_serde records -> coalesced columns
+constexpr int IPC_TILE = 1024;                 // rows of one (record, column) tile of ipc_decode_fixed_kernel
+constexpr int IPC_COPY_PIECE = 32768;          // bytes of one piece of ipc_decode_bytes_kernel
+struct IpcFixedJob { const uint8_t* src; uint8_t* dst; int64_t rows; int32_t width; int32_t _pad; };   // src: `width` planes; dst: the record's first output value
+struct IpcTile { int32_t job; int32_t row0; };
+struct IpcBitCol { uint32_t* dst; const uint8_t* const* src; };   // src: per record, its bitmap in the stream, or null (all bits set)
+struct IpcCopy { const uint8_t* src; uint8_t* dst; int64_t len; };
+int launch_ipc_decode_fixed(const IpcFixedJob* jobs, const IpcTile* tiles, int64_t ntiles, cudaStream_t s);
+int launch_ipc_decode_bits(const IpcBitCol* cols, int ncols, const int64_t* rec_row /* nrec + 1 output row starts */, int64_t nrec, int64_t rows, cudaStream_t s);
+int launch_ipc_decode_bytes(const IpcCopy* copies, int64_t n, cudaStream_t s);
+
 }  // namespace b200q

@@ -100,6 +100,8 @@ DevMemP upload(OpContext& cx, const void* p, size_t n, size_t pad = 16) {
 
 // host half of one column chunk (runs on a worker thread): read, frame + decompress the pages, flatten them into one byte buffer and
 // two run tables (levels by row, values by stored-value ordinal)
+}  // namespace
+
 // Pinned host blocks outlive a scan: pinning pages costs ~1 ms per MB and a long-lived executor runs scan after scan.  Process-wide pool of
 // power-of-two blocks, bounded in bytes (B200Q_SCAN_HOST_CACHE_MB, default 2048); blocks above the bound go back to the driver.
 struct PinnedPool {
@@ -121,6 +123,8 @@ struct PinnedPool {
 PinnedPool& pinned_pool() { static PinnedPool* p = new PinnedPool(); return *p; }            // leaked on purpose: no pinned frees after the driver is gone
 void* pinned_alloc(size_t n) { return pinned_pool().get(n); }
 void pinned_free(void* p) { pinned_pool().put(p); }
+
+namespace {
 
 // host half of one column chunk: the file bytes, the decompressed page bodies (what the device reads) and the run tables
 struct PreparedChunk {

@@ -393,6 +393,35 @@ PlanP parse_leaf(Reader r, bool ffi) {
   return n;
 }
 
+// IpcReaderExecNode{num_partitions=1, schema=2, ipc_provider_resource_id=3} (auron.proto:607-611; from_proto.rs IpcReader arm): the
+// reduce side of a shuffle.  Its columns are what batch_serde writes and the device carries (Utf8 has Binary's wire form,
+// batch_serde.rs:129-131,180-181); the writer refuses Null columns (shuffle_stage.cu), so does the reader.
+PlanP parse_ipc_reader(Reader r) {
+  auto n = std::make_shared<PlanNode>(); n->kind = N_LEAF; n->leaf_kind = "IpcReader";
+  bool have = false;
+  while (!r.done()) {
+    int wt; uint32_t f = r.tag(wt);
+    if (f == 2) {
+      Reader s = r.bytes(); have = true;
+      while (!s.done()) {
+        int w2; uint32_t g = s.tag(w2);
+        if (g != 1) { s.skip(w2); continue; }
+        Reader fr = s.bytes();
+        std::string name;
+        { Reader nr = fr; while (!nr.done()) { int w3; uint32_t h = nr.tag(w3); if (h == 1) name = nr.str(); else nr.skip(w3); } }
+        FieldDef fd;
+        try { fd = parse_field(fr); }
+        catch (const PlanError& e) { if (e.code == B200Q_ERR_UNSUPPORTED) unsupported("IpcReaderExec: column " + name + ": " + e.what()); throw; }
+        if (fd.type.id == T_NULL) unsupported("IpcReaderExec: column " + fd.name + " is Null; the shuffle writer does not write Null columns");
+        n->schema.fields.push_back(fd);
+      }
+    } else if (f == 3) n->resource_id = r.str();
+    else r.skip(wt);
+  }
+  if (!have) bad("leaf node without schema");
+  return n;
+}
+
 // ParquetScanExecNode{base_conf=1, pruning_predicates=2, fsResourceId=3}; FileScanExecConf{num_partitions=1, partition_index=2, file_group=3,
 // schema=4, projection=6, limit=7, statistics=8, partition_schema=9} (auron.proto:404-419; from_proto.rs ParquetScan arm)
 PlanP parse_parquet_scan(Reader r) {
@@ -813,6 +842,7 @@ PlanP parse_plan(Reader r) {                  // PhysicalPlanNode oneof (auron.p
     int wt; uint32_t f = r.tag(wt);
     switch (f) {
       case 2: return parse_shuffle_writer(r.bytes());
+      case 3: return parse_ipc_reader(r.bytes());
       case 5: return parse_parquet_scan(r.bytes());
       case 6: return parse_projection(r.bytes());
       case 7: return parse_sort(r.bytes());
@@ -825,7 +855,7 @@ PlanP parse_plan(Reader r) {                  // PhysicalPlanNode oneof (auron.p
       case 18: return parse_leaf(r.bytes(), true);
       case 20: return parse_expand(r.bytes());
       case 22: return parse_window(r.bytes());
-      case 1: case 3: case 4: case 9: case 10: case 14: case 17: case 19:
+      case 1: case 4: case 9: case 10: case 14: case 17: case 19:
       case 21: case 23: case 24: case 25:
         unsupported("plan node #" + std::to_string(f) + " is outside the Filter/Project/Agg hot path (SURVEY.md §8)");
       default: r.skip(wt);

@@ -119,6 +119,22 @@ struct ShuffleResult {
 // ParquetScanExec (parquet_source.cu): the source of an op whose leaf is a ParquetScanExecNode; `emit` receives one device batch per row group
 void run_parquet_scan(OpContext& cx, const PlanNode& leaf, const std::function<void(DevBatch&)>& emit);
 void set_file_reader(b200q_file_reader_fn fn, void* ctx);
+// the process-wide pool of pinned host blocks (parquet_source.cu) the scan and the IpcReaderExec source stage their bytes in;
+// pinned_alloc returns null when the driver refuses the allocation
+void* pinned_alloc(size_t n);
+void pinned_free(void* p);
+
+// IpcReaderExec (ipc_source.cu): the source of an op whose leaf is an IpcReaderExecNode.  push() takes the bytes of one BlockObject
+// (`u32 LE length ‖ LZ4 frame` blocks), decompresses them on host threads into pinned blocks, walks their batch_serde records and
+// uploads them; the records accumulate into one device batch of up to conf.staging_rows rows, decoded on the device and handed to
+// `emit` (at push when full, at flush otherwise).  Malformed input -> ExecError(INVALID_ARG) before anything of the push is kept.
+class IpcSource {
+ public:
+  virtual ~IpcSource() {}
+  virtual void push(OpContext& cx, const uint8_t* data, size_t len, const std::function<void(DevBatch&)>& emit) = 0;
+  virtual void flush(OpContext& cx, const std::function<void(DevBatch&)>& emit) = 0;
+};
+std::unique_ptr<IpcSource> make_ipc_source(OpContext& cx, const SchemaDef& schema, const std::vector<int>& used_cols);
 
 // SortExec (sort_stage.cu): collects its input, emits the sorted (and `fetch`-limited) rows at finish
 std::unique_ptr<Stage> make_sort_stage(OpContext& cx, const SchemaDef& in_schema, const PlanNode& node);

@@ -77,6 +77,7 @@ SYMBOLS = ["b200q_version", "b200q_build_info", "b200q_last_error", "b200q_devic
            "b200q_op_push_device", "b200q_op_finish", "b200q_op_pull", "b200q_op_pull_device", "b200q_op_sync",
            "b200q_op_metrics", "b200q_op_destroy", "b200q_murmur3_partition",
            "b200q_set_file_reader", "b200q_parquet_explain", "b200q_snappy_uncompress", "b200q_op_attach_build", "b200q_op_shuffle_chunk_count", "b200q_op_shuffle_chunk", "b200q_lz4_frame_compress",
+           "b200q_lz4_frame_decompress", "b200q_op_push_ipc",
            "b200q_exchange_unique_id", "b200q_exchange_create", "b200q_exchange_shuffle", "b200q_exchange_kernel_launches",
            "b200q_exchange_destroy"]
 
@@ -112,6 +113,8 @@ def _load():
     lib.b200q_op_shuffle_chunk_count.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
     lib.b200q_op_shuffle_chunk.argtypes = [C.c_void_p, C.c_int64, C.POINTER(ShuffleChunk)]
     lib.b200q_lz4_frame_compress.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    lib.b200q_lz4_frame_decompress.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    lib.b200q_op_push_ipc.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]
     lib.b200q_exchange_unique_id.argtypes = [C.c_void_p]
     lib.b200q_exchange_create.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
     lib.b200q_exchange_shuffle.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
@@ -147,6 +150,17 @@ def lz4_frame_compress(data: bytes) -> bytes:
     cap = len(data) + len(data) // 255 + 64
     buf = C.create_string_buffer(cap)
     check(lib.b200q_lz4_frame_compress(data, len(data), buf, cap, C.byref(need)))
+    return buf.raw[: need.value]
+
+
+def lz4_frame_decompress(data: bytes) -> bytes:
+    """the library's own LZ4 frame decoder (host only): the compression blocks the reduce side reads"""
+    need = C.c_size_t(0)
+    st = lib.b200q_lz4_frame_decompress(data, len(data), None, 0, C.byref(need))
+    if st != ERR_INVALID_ARG or "needs" not in last_error():
+        check(st)
+    buf = C.create_string_buffer(max(1, need.value))
+    check(lib.b200q_lz4_frame_decompress(data, len(data), buf, need.value, C.byref(need)))
     return buf.raw[: need.value]
 
 
@@ -266,6 +280,10 @@ class NativeOp:
         finally:
             import pyarrow as pa
             pa.Schema._import_from_c(C.addressof(s))     # releases the exported schema
+
+    def push_ipc(self, data: bytes):
+        """IpcReaderExec leaves: the bytes of one BlockObject (`u32 LE length ‖ LZ4 frame` blocks)"""
+        check(lib.b200q_op_push_ipc(self._h, data, len(data)))
 
     def push_device(self, batch: DeviceBatch):
         check(lib.b200q_op_push_device(self._h, C.addressof(batch.dev)))

@@ -61,7 +61,7 @@ class ExecutionPlan:
         leaf = self.leaf()
         with native.NativeOp(self.plan_bytes(), conf, device) as op:
             for rb in leaf.batches:
-                op.push(rb)
+                leaf.push_to(op, rb)
                 while True:
                     out = op.pull()
                     if out is None:
@@ -102,6 +102,31 @@ class MemoryExec(ExecutionPlan):
 
     def node(self):
         return P.ffi_reader_node(self._schema, self.resource_id)
+
+    @staticmethod
+    def push_to(op: native.NativeOp, rb):
+        op.push(rb)
+
+
+class IpcReaderExec(ExecutionPlan):
+    """IpcReaderExec::new(num_partitions, ipc_provider_resource_id, schema) (ipc_reader_exec.rs:64-80): the reduce side of a
+    shuffle.  `blocks` plays the role of the BlockObjects the provider yields: each element is the bytes of one (a concatenation of
+    `u32 LE length ‖ LZ4 frame` blocks, e.g. one map output's byte range of a partition) and is handed to the op with push_ipc."""
+
+    def __init__(self, schema: Schema, blocks: Sequence[bytes] = (), num_partitions: int = 1, resource_id: str = ""):
+        self._schema, self.num_partitions, self.resource_id = schema, num_partitions, resource_id
+        self.batches = [bytes(b) for b in blocks]
+        self._validate()
+
+    def schema(self):
+        return self._schema
+
+    def node(self):
+        return P.ipc_reader_node(self._schema, self.resource_id, self.num_partitions)
+
+    @staticmethod
+    def push_to(op: native.NativeOp, block: bytes):
+        op.push_ipc(block)
 
 
 class FilterExec(ExecutionPlan):
@@ -346,13 +371,13 @@ class BroadcastJoinExec(ExecutionPlan):
         build_plan = BroadcastJoinBuildHashMapExec(data, keys)
         with native.NativeOp(build_plan.plan_bytes(), conf, device) as bop:
             for rb in data.leaf().batches:
-                bop.push(rb)
+                data.leaf().push_to(bop, rb)
             bop.finish()
             self.build_metrics = bop.metrics()
             with native.NativeOp(self.plan_bytes(), conf, device) as op:
                 op.attach_build(bop)
                 for rb in probe.leaf().batches:
-                    op.push(rb)
+                    probe.leaf().push_to(op, rb)
                     yield from op.pull_all()
                 op.finish()
                 yield from op.pull_all()
@@ -386,7 +411,7 @@ class ShuffleWriterExec(ExecutionPlan):
         leaf = self.leaf()
         with native.NativeOp(self.plan_bytes(), conf, device) as op:
             for rb in leaf.batches:
-                op.push(rb)
+                leaf.push_to(op, rb)
             op.finish()
             self.last_chunks = op.shuffle_chunks()
             self.last_metrics = op.metrics()

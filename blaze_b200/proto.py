@@ -178,7 +178,7 @@ def _build_pool():
         ("broadcast_join", 13, "BroadcastJoinExecNode", O), ("filter", 8, "FilterExecNode", O),
         ("empty_partitions", 15, "EmptyPartitionsExecNode", O), ("agg", 16, "AggExecNode", O),
         ("ffi_reader", 18, "FFIReaderExecNode", O), ("expand", 20, "PhysicalPlanNode.ExpandExecNode", O),
-        ("window", 22, "PhysicalPlanNode.WindowExecNode", O),
+        ("window", 22, "PhysicalPlanNode.WindowExecNode", O), ("ipc_reader", 3, "PhysicalPlanNode.IpcReaderExecNode", O),
     ], oneofs=["PhysicalPlanType"])
     # ExpandExecNode{input=1, schema=2, projections=3} and ExpandProjection{expr=1} (auron.proto:714-722) are top-level in the reference;
     # nested here like the string-match nodes above (same bytes on the wire), the top-level set stays that of the field table of
@@ -203,6 +203,10 @@ def _build_pool():
                                 ("window_func", 3, "enum:PhysicalPlanNode.WindowFunction"), ("agg_func", 4, "enum:AggFunction"),
                                 ("children", 5, "PhysicalExprNode", R)], into=pp.nested_type)
     _msg(fd, "WindowGroupLimit", [("k", 1, _F.TYPE_UINT32)], into=pp.nested_type)
+    # IpcReaderExecNode (auron.proto:607-611): nested the same way; tests/test_proto_ipc_reader_compat.py checks it against
+    # tests/golden/auron_proto_ipc_reader_fields.json
+    _msg(fd, "IpcReaderExecNode", [("num_partitions", 1, _F.TYPE_UINT32), ("schema", 2, "Schema"), ("ipc_provider_resource_id", 3, _F.TYPE_STRING)],
+         into=pp.nested_type)
     _msg(fd, "PartitionId", [("stage_id", 2, _F.TYPE_UINT32), ("partition_id", 4, _F.TYPE_UINT32), ("task_id", 5, _F.TYPE_UINT64)])
     _msg(fd, "TaskDefinition", [("task_id", 1, "PartitionId"), ("plan", 2, "PhysicalPlanNode")])
 
@@ -361,6 +365,14 @@ def ffi_reader_node(schema: Schema, resource_id: str = "", num_partitions: int =
     n.ffi_reader.num_partitions = num_partitions
     n.ffi_reader.schema.CopyFrom(schema_msg(schema))
     n.ffi_reader.export_iter_provider_resource_id = resource_id
+    return n
+
+
+def ipc_reader_node(schema: Schema, resource_id: str = "", num_partitions: int = 1):
+    n = PhysicalPlanNode()
+    n.ipc_reader.num_partitions = num_partitions
+    n.ipc_reader.schema.CopyFrom(schema_msg(schema))
+    n.ipc_reader.ipc_provider_resource_id = resource_id
     return n
 
 

@@ -39,6 +39,7 @@
  *   ParquetScanExecNode leaf ParquetExec::execute (decode + row-group pruning)      datafusion-ext-plans/src/parquet_exec.rs:150-203,316-396
  *   SortExecNode plans      SortExec::new + ExternalSorter::insert_batch / output   datafusion-ext-plans/src/sort_exec.rs:97-112,626-752
  *   b200q_op_attach_build   collect_join_hash_map + execute_join_with_map   datafusion-ext-plans/src/broadcast_join_exec.rs:317-385,562-639
+ *   b200q_op_push_ipc       IpcReaderExec::execute (decode of the shuffle blocks)  datafusion-ext-plans/src/ipc_reader_exec.rs:164-272
  *   b200q_op_shuffle_chunk  the per-partition encoded bytes before compression — what BufferedData::write_rss
  *                           hands to an RSS partition writer (buffered_data.rs:160-196)
  *
@@ -275,6 +276,23 @@ b200q_status b200q_op_shuffle_chunk(b200q_op* op, int64_t index, b200q_shuffle_c
  * appends one frame holding src[0, n) to dst (capacity cap); *out_len = frame bytes, or the bytes needed when
  * the call fails with B200Q_ERR_INVALID_ARG because cap is too small. */
 b200q_status b200q_lz4_frame_compress(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, size_t* out_len);
+/* The library's LZ4 frame decoder (host only, no GPU needed): decodes the concatenated frame(s) src[0, n) into dst (capacity
+ * cap); *out_len = decoded bytes, or the bytes needed when the call fails with B200Q_ERR_INVALID_ARG because cap is too small.
+ * Any frame the LZ4 frame format does not allow (bad magic, reserved bits, truncation, a match before the output start, an
+ * overrun, a checksum mismatch) is B200Q_ERR_INVALID_ARG with the byte offset in the message. */
+b200q_status b200q_lz4_frame_decompress(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, size_t* out_len);
+
+/* ---- IpcReaderExec as the source of an op (plans whose leaf is an IpcReaderExecNode) ------------------------------------
+ * Reference: IpcReaderExec::execute (datafusion-ext-plans/src/ipc_reader_exec.rs:164-272), IpcCompressionReader
+ * (common/ipc_compression.rs:114-183) and read_batch (datafusion-ext-commons/src/io/batch_serde.rs:79-99).  Such an op takes
+ * no b200q_op_push / b200q_op_push_device (B200Q_ERR_STATE); each call hands over the bytes of one BlockObject: a
+ * concatenation of `u32 LE length ‖ LZ4 frame` blocks, e.g. one map output's byte range of this partition as its .index file
+ * gives it.  The records of consecutive pushes are coalesced into device batches of up to conf.staging_rows rows (b200q_op_finish
+ * decodes the rest); a record may straddle two blocks of one push but not two pushes.  The library has finished reading `data`
+ * when the call returns.  Malformed bytes -> B200Q_ERR_INVALID_ARG (what is wrong, at which byte of the push); nothing of that
+ * push is kept and the handle stays usable.  A zstd frame -> B200Q_ERR_UNSUPPORTED.  b200q_op_push_ipc on an op with another
+ * leaf -> B200Q_ERR_STATE. */
+b200q_status b200q_op_push_ipc(b200q_op* op, const uint8_t* data, size_t len);
 
 /* Spark-compatible partition ids of device-resident key columns:
  * pid[i] = pmod(murmur3_x86_32 chained over the key columns (NULL leaves the hash unchanged), seed 42,

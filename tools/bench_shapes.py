@@ -618,3 +618,157 @@ if any(t in (ONLY or "F1,F2") for t in ("F1", "F2")):
                               "power_limit": plim, "rows": frows, "out_rows": n_out, "verified_groups": n_out == n_keys, "wall_ms_push_to_sync": dt * 1e3,
                               "rows_per_s": frows / dt, "wall_ms_all_runs": [round(x[0] * 1e3, 2) for x in res[v]], "fast_path_launches": m["fast_path_launches"],
                               "launches": m["gpu_kernel_launches"]}), flush=True)
+
+
+# R1-R2: IpcReaderExec, the reduce side of a shuffle (DESIGN §3.13).  The map side writes reference-format shuffle files on the GPU
+# (ShuffleWriterExec); the reduce side reads them back with IpcReader ops.
+# R1 is q1's reduce side: 8 map ops of Filter -> AggExec(Partial) -> ShuffleWriterExec(hash, 200) over 2^26 rows in total (k ~ U[0, 2^20));
+# then, per reduce partition, IpcReader -> AggExec(Final) over that partition's byte range of every map output, timed whole-op from the
+# first push_ipc to sync (summed over the partitions).  In the same call the same rows, decoded beforehand, go through push (the FFI path
+# today) into the same AggExec(Final): a lower bound of the current path, which also pays a CPU decode not timed here.
+# R2 is the decode rate: a single-partition shuffle of 2^26 rows of [k int64, v int64, x float64, d decimal128, b bool] with 10 % NULLs
+# read back by a bare IpcReader op, split into host LZ4 decompression (the op's block decoder on as many threads), the H2D copy of the
+# decompressed bytes, the ipc_decode_* kernels (torch.profiler, a run of its own) and the whole op.
+def _partition_ranges(data_path, index_path):
+    import struct as _st
+    data, index = open(data_path, "rb").read(), open(index_path, "rb").read()
+    offs = _st.unpack("<%dq" % (len(index) // 8), index)
+    return [data[offs[i]: offs[i + 1]] for i in range(len(offs) - 1)]
+
+
+if any(t in (ONLY or "R1,R2") for t in ("R1", "R2")):
+    import subprocess, tempfile, time
+    import numpy as np
+    import pyarrow as pa
+    card = torch.cuda.get_device_name(0)
+    try:
+        plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True).stdout.strip()
+    except OSError:
+        plim = "unknown"
+    rrows = int(os.environ.get("ROWS", 1 << 26))
+    tmp = tempfile.mkdtemp(prefix="b200q_ipc_")
+    if "R1" in (ONLY or "R1"):
+        P, M = 200, 8
+        r_sch = T.Schema([T.Field("k", T.int64, False), T.Field("v", T.int64, False)])
+        r_g = [E.GroupingExpr("k", E.Column("k"))]
+        r_aggs = lambda mode, ins: [E.AggExpr("s", mode, PL.create_agg(E.AGG_SUM, [E.Column("v") if mode == E.PARTIAL else E.placeholder(T.int64)], ins, T.int64)),
+                                    E.AggExpr("c", mode, PL.create_agg(E.AGG_COUNT, [E.Column("v") if mode == E.PARTIAL else E.placeholder(T.int64)], ins, T.int64))]
+        preds = [E.BinaryExpr(E.Column("v"), "Lt", E.Literal(0, T.int64))]
+        partial = PL.AggExec(PL.HashAgg, r_g, r_aggs(E.PARTIAL, r_sch), False, PL.FilterExec(preds, PL.MemoryExec(r_sch)))
+        pschema = partial.schema()
+        per = rrows // M
+        files, kept = [], []
+        for m in range(M):
+            k = torch.randint(0, 1 << 20, (per,), dtype=torch.int64, device=dev, generator=g)
+            v = torch.randint(-10**6, 10**6, (per,), dtype=torch.int64, device=dev, generator=g)
+            kept.append(torch.unique(k[v < 0]))
+            w = PL.ShuffleWriterExec(partial, ("hash", [E.Column("k")], P), os.path.join(tmp, f"m{m}.data"), os.path.join(tmp, f"m{m}.index"))
+            with native.NativeOp(w.plan_bytes(), native.default_conf(), 0) as op:
+                op.push_device(native.DeviceBatch([(k.data_ptr(), 0, per), (v.data_ptr(), 0, per)], per, 0, keepalive=(k, v)))
+                op.finish()
+            files.append(_partition_ranges(w.output_data_file, w.output_index_file))
+        n_groups = int(torch.unique(torch.cat(kept)).numel())
+        final_of = lambda leaf: PL.AggExec(PL.HashAgg, r_g, r_aggs(E.FINAL, pschema), False, leaf)
+        ipc_plan = final_of(PL.IpcReaderExec(pschema)).plan_bytes()
+        ffi_plan = final_of(PL.MemoryExec(pschema)).plan_bytes()
+        decoded = []                                       # each partition's rows, decoded once beforehand (host Arrow batches)
+        for q in range(P):
+            with native.NativeOp(PL.IpcReaderExec(pschema).plan_bytes(), native.default_conf(), 0) as op:
+                for f in files:
+                    op.push_ipc(f[q])
+                op.finish()
+                decoded.append(op.pull_all())
+        def reduce_side(ipc):
+            t, out = 0.0, []
+            for q in range(P):
+                with native.NativeOp(ipc_plan if ipc else ffi_plan, native.default_conf(), 0) as op:
+                    t0 = time.perf_counter()
+                    if ipc:
+                        for f in files:
+                            op.push_ipc(f[q])
+                    else:
+                        for b in decoded[q]:
+                            op.push(b)
+                    op.finish(); op.sync()
+                    t += time.perf_counter() - t0
+                    out += op.pull_all()
+            return t, out
+        reduce_side(True); reduce_side(False)               # warm-up
+        ti, tf = [], []
+        for _ in range(REPS or 3):                           # alternated in this call
+            a, out_ipc = reduce_side(True); ti.append(a)
+            b, out_ffi = reduce_side(False); tf.append(b)
+        canon = lambda bs: sorted(zip(*[pa.concat_arrays([x.column(i) for x in bs]).to_pylist() for i in range(3)]))
+        got_ipc, got_ffi = canon(out_ipc), canon(out_ffi)
+        print(json.dumps({"shape": "R1 q1 reduce side: per partition IpcReader -> AggExec(Final), 8 map outputs x 200 partitions", "card": card,
+                          "power_limit": plim, "rows": rrows, "groups": len(got_ipc), "map_bytes": sum(len(x) for f in files for x in f),
+                          "verified": got_ipc == got_ffi and len(got_ipc) == n_groups,
+                          "wall_ms_ipc_all_partitions": min(ti) * 1e3, "wall_ms_ffi_push_all_partitions": min(tf) * 1e3,
+                          "wall_ms_ipc_runs": [round(x * 1e3, 1) for x in ti], "wall_ms_ffi_runs": [round(x * 1e3, 1) for x in tf]}), flush=True)
+        del decoded
+    if "R2" in (ONLY or "R2"):
+        rng = np.random.default_rng(5)
+        n = rrows
+        cols_np = {"k": rng.integers(-2**62, 2**62, n), "v": rng.integers(-10**9, 10**9, n), "x": rng.normal(0, 1e6, n)}
+        d = torch.randint(-2**62, 2**62, (n, 2), dtype=torch.int64, device=dev, generator=g)
+        bvals = torch.randint(0, 256, ((n + 7) // 8,), dtype=torch.uint8, device=dev, generator=g)
+        valid = [torch.from_numpy(np.packbits(rng.random(n) >= 0.1, bitorder="little")).to(dev) for _ in range(5)]
+        tk, tv, tx = (torch.from_numpy(cols_np[c]).to(dev) for c in ("k", "v", "x"))
+        s2 = T.Schema([T.Field("k", T.int64, True), T.Field("v", T.int64, True), T.Field("x", T.float64, True),
+                       T.Field("d", T.decimal128(38, 2), True), T.Field("b", T.bool_, True)])
+        w = PL.ShuffleWriterExec(PL.MemoryExec(s2), ("single",), os.path.join(tmp, "r2.data"), os.path.join(tmp, "r2.index"))
+        with native.NativeOp(w.plan_bytes(), native.default_conf(), 0) as op:
+            op.push_device(native.DeviceBatch([(t.data_ptr(), vb.data_ptr(), n) for t, vb in zip([tk, tv, tx, d, bvals], valid)], n, 0,
+                                              keepalive=[tk, tv, tx, d, bvals] + valid))
+            op.finish()
+        part = _partition_ranges(w.output_data_file, w.output_index_file)[0]
+        bare = PL.IpcReaderExec(s2).plan_bytes()
+        def whole_op(pull=False):
+            with native.NativeOp(bare, native.default_conf(), 0) as op:
+                torch.cuda.synchronize(); t0 = time.perf_counter()
+                op.push_ipc(part)
+                op.finish(); op.sync()
+                dt = time.perf_counter() - t0
+                return dt, op.metrics(), (op.pull_all() if pull else None)
+        whole_op()
+        walls = [whole_op()[0] for _ in range(REPS or 3)]
+        # host half alone: the same block decoder over the same blocks, on as many threads as the op uses
+        import struct as _st
+        from concurrent.futures import ThreadPoolExecutor
+        blocks, pos = [], 0
+        while pos < len(part):
+            (bl,) = _st.unpack_from("<I", part, pos); blocks.append(part[pos + 4: pos + 4 + bl]); pos += 4 + bl
+        nthreads = min(os.cpu_count() or 1, 32, len(blocks))
+        with ThreadPoolExecutor(nthreads) as ex:
+            list(ex.map(native.lz4_frame_decompress, blocks[:nthreads]))
+            t0 = time.perf_counter(); payload = sum(len(x) for x in ex.map(native.lz4_frame_decompress, blocks)); t_lz4 = time.perf_counter() - t0
+        pinned = torch.empty(payload, dtype=torch.uint8).pin_memory()
+        dbuf = torch.empty(payload, dtype=torch.uint8, device=dev)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        dbuf.copy_(pinned, non_blocking=True); torch.cuda.synchronize()
+        e0.record(); dbuf.copy_(pinned, non_blocking=True); e1.record(); torch.cuda.synchronize()
+        t_h2d = e0.elapsed_time(e1) / 1e3
+        del pinned, dbuf
+        from torch.profiler import profile, ProfilerActivity
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            whole_op()
+        k_us = sum(e.device_time_total for e in prof.key_averages() if "ipc_decode" in e.key)
+        out_bytes = n * (8 + 8 + 8 + 16) + 6 * ((n + 31) // 32) * 4         # values, 5 validity bitmaps and the Boolean values
+        alg = payload + out_bytes                                            # every encoded byte read once, every value byte written once
+        dt, m, out = whole_op(pull=True)
+        ok = True
+        for ci, name in ((0, "k"), (1, "v")):                                # the writer places a partition's rows in any order: compare multisets
+            got = pa.concat_arrays([b.column(ci) for b in out])
+            kv = np.unpackbits(valid[ci].cpu().numpy(), bitorder="little")[:n].astype(bool)
+            gv = np.asarray(got.is_valid())
+            vals = np.frombuffer(got.buffers()[1], np.int64, count=len(got), offset=got.offset * 8)
+            ok = ok and len(got) == n and int(gv.sum()) == int(kv.sum()) and np.array_equal(np.sort(vals[gv]), np.sort(cols_np[name][kv]))
+        print(json.dumps({"shape": "R2 IpcReader decode of 2^26 rows [k i64, v i64, x f64, d dec128, b bool], 10% NULLs", "card": card, "power_limit": plim,
+                          "rows": n, "compressed_bytes": len(part), "decompressed_bytes": payload, "blocks": len(blocks), "verified": bool(ok),
+                          "host_lz4_ms": t_lz4 * 1e3, "host_lz4_threads": nthreads, "h2d_ms": t_h2d * 1e3, "h2d_GBps": payload / t_h2d / 1e9,
+                          "ipc_decode_kernels_ms": k_us / 1e3, "ipc_decode_alg_bytes": alg,
+                          "ipc_decode_frac_of_hbm_peak": (alg / (k_us / 1e6) / 1e9 / peak) if k_us else None,
+                          "wall_ms_whole_op": min(walls) * 1e3, "wall_ms_runs": [round(x * 1e3, 1) for x in walls],
+                          "launches": m["gpu_kernel_launches"], "elapsed_compute_ms": m["elapsed_compute_ns"] / 1e6}), flush=True)
+    import shutil
+    shutil.rmtree(tmp, ignore_errors=True)

@@ -1,4 +1,5 @@
-"""Seed plans for tools/fuzz/plan_decode_fuzz.cc: every node / expression kind the decoder accepts."""
+"""Seeds for tools/fuzz: plans with every node / expression kind the decoder accepts (plan_decode_fuzz.cc); LZ4 frames written by the
+library and by liblz4 (pyarrow) and batch_serde record streams over random schemas written by the oracle (ipc_fuzz.cc)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 from blaze_b200 import exprs as E, plans as PL, types as T
@@ -55,3 +56,35 @@ if __name__ == "__main__":
             ("abc", T.utf8), ("", T.utf8), (None, T.utf8), ("h\u00e9\u20ac\U0001F600" * 9, T.utf8)]
     for i, (v, dt) in enumerate(lits):
         open(os.path.join(out, "lit%d.bin" % i), "wb").write(proto.literal_ipc_bytes(v, dt))
+    # LZ4 frames (ipc_fuzz --lz4): the library's encoder and liblz4 over byte planes, text, zeros and noise
+    import numpy as np
+    import pyarrow as pa
+    from blaze_b200 import native
+    rng = np.random.default_rng(3)
+    datas = [b"", b"x", b"abcabcabcabca" * 9, np.frombuffer(rng.integers(-10**6, 10**6, 4000, dtype=np.int64).tobytes(), np.uint8).reshape(-1, 8).T.tobytes(),
+             bytes(70_000), rng.integers(0, 256, 3000, dtype=np.uint8).tobytes()]
+    for i, d in enumerate(datas):
+        open(os.path.join(out, "lz4_lib%d.bin" % i), "wb").write(native.lz4_frame_compress(d))
+        open(os.path.join(out, "lz4_pa%d.bin" % i), "wb").write(pa.Codec("lz4").compress(d, asbytes=True))
+    # record streams (ipc_fuzz --records): [ncols][type ids][records], every type, with and without NULLs
+    from oracle import blaze_oracle as O, shuffle_oracle as S
+    cases = [[("a", pa.int64(), T.INT64), ("b", pa.binary(), T.BINARY)], [("c", pa.bool_(), T.BOOL), ("d", pa.int16(), T.INT16), ("e", pa.float64(), T.FLOAT64)],
+             [("f", pa.decimal128(20, 2), T.DECIMAL128), ("g", pa.int32(), T.INT32), ("h", pa.binary(), T.BINARY), ("i", pa.int8(), T.INT8)]]
+    for i, cols in enumerate(cases):
+        raw = b""
+        for n in (1, 7, 33):
+            arrays = []
+            for name, pt, tid in cols:
+                mask = rng.random(n) < 0.3
+                if tid == T.BINARY:
+                    arrays.append(pa.array([None if m else bytes(rng.integers(0, 256, int(rng.integers(0, 9)), dtype=np.uint8)) for m in mask], pt))
+                elif tid == T.BOOL:
+                    arrays.append(pa.array(rng.random(n) < 0.5, pt, mask=mask))
+                elif tid == T.DECIMAL128:
+                    import decimal
+                    arrays.append(pa.array([None if m else decimal.Decimal(int(rng.integers(-10**9, 10**9))).scaleb(-2) for m in mask], pt))
+                else:
+                    arrays.append(pa.array(np.where(mask, 0, rng.integers(-100, 100, n)).astype(pt.to_pandas_dtype()), pt, mask=mask))
+            b = O.batch_from_arrow(pa.RecordBatch.from_arrays(arrays, names=[c[0] for c in cols]))
+            raw += S.write_batch(n, b.cols)
+        open(os.path.join(out, "rec_%d.bin" % i), "wb").write(bytes([len(cols)] + [c[2] for c in cols]) + raw)
