@@ -100,6 +100,7 @@ struct b200q_op {
   cudaEvent_t ev_a = nullptr, ev_b = nullptr;
   std::shared_ptr<StreamRef> stream_ref;
   std::unique_ptr<IpcSource> ipc;   // the op's source when its leaf is an IpcReaderExecNode (input through b200q_op_push_ipc only)
+  bool taken = false;               // its output became the right side of a sort-merge join (b200q_op_attach_right)
 };
 
 namespace b200q {
@@ -122,6 +123,16 @@ static b200q_status guarded(b200q_op* op, F&& f) {
   } catch (const std::exception& e) { return fail(B200Q_ERR_EXECUTION, e.what()); }
 }
 b200q_status guarded_call(const std::function<void()>& f) { return guarded(nullptr, f); }
+
+static SmjRightAttach* smj_of(b200q_op* op) {
+  for (auto& st : op->stages) if (auto* j = dynamic_cast<SmjRightAttach*>(st.get())) return j;
+  return nullptr;
+}
+// a sort-merge join op takes no input before its right side is attached
+static void require_right_side(b200q_op* op) {
+  const SmjRightAttach* j = smj_of(op);
+  if (j && !j->right_attached()) throw ExecError(B200Q_ERR_STATE, "SortMergeJoinExec: attach the right side (b200q_op_attach_right) before the first push or finish");
+}
 
 // ---- pipeline construction ----------------------------------------------------------------------------
 static std::vector<ExprP> identity_cols(const SchemaDef& s) {
@@ -282,6 +293,13 @@ static void build_pipeline(b200q_op* op) {
         op->stages.push_back(make_join_probe_stage(op->cx, stage_in, *n));
         stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in);
       }
+    } else if (n->kind == N_SMJ) {
+      if (pending_tail) {                               // Filter / Project chain below the left side: its own fused stage
+        op->stages.push_back(make_filter_project_stage(op->cx, stage_in, filters, cur_cols, n->input->schema));
+        stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in); filters.clear(); pending_tail = false;
+      }
+      op->stages.push_back(make_smj_stage(op->cx, stage_in, *n));
+      stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in);
     } else if (n->kind == N_SHUFFLE_WRITER) {
       if (i + 1 != chain.size()) throw PlanError(B200Q_ERR_UNSUPPORTED, "ShuffleWriterExec below another operator");
       if (pending_tail) {                               // Filter / Project chain below the writer: its own fused stage
@@ -687,6 +705,7 @@ b200q_status b200q_op_push(b200q_op* op, struct ArrowArray* batch) {
   b200q_status st = guarded(op, [&] {
     if (op->finished) throw ExecError(B200Q_ERR_STATE, "push after finish");
     if (op->ipc) throw ExecError(B200Q_ERR_STATE, "an op whose leaf is an IpcReaderExecNode takes its input through b200q_op_push_ipc");
+    require_right_side(op);
     B200Q_CUDA(cudaSetDevice(op->cx.device));
     validate_host_batch(op, batch);
     poll_pending(op, false);
@@ -714,6 +733,7 @@ b200q_status b200q_op_push_ipc(b200q_op* op, const uint8_t* data, size_t len) {
     if (op->finished) throw ExecError(B200Q_ERR_STATE, "push after finish");
     if (!op->ipc) throw ExecError(B200Q_ERR_STATE, "push_ipc: the op's leaf is not an IpcReaderExecNode");
     if (!data && len) throw ExecError(B200Q_ERR_INVALID_ARG, "push_ipc: null data");
+    require_right_side(op);
     B200Q_CUDA(cudaSetDevice(op->cx.device));
     poll_pending(op, false);
     op->ipc->push(op->cx, data, len, [&](DevBatch& b) { run_stages(op, b, 0); });
@@ -727,6 +747,7 @@ b200q_status b200q_op_push_device(b200q_op* op, struct ArrowDeviceArray* dbatch)
     if (op->ipc) throw ExecError(B200Q_ERR_STATE, "an op whose leaf is an IpcReaderExecNode takes its input through b200q_op_push_ipc");
     if (!dbatch) throw ExecError(B200Q_ERR_INVALID_ARG, "null batch");
     if (dbatch->device_type != ARROW_DEVICE_CUDA || dbatch->device_id != op->cx.device) throw ExecError(B200Q_ERR_INVALID_ARG, "push_device: batch is not on this op's CUDA device");
+    require_right_side(op);
     B200Q_CUDA(cudaSetDevice(op->cx.device));
     ArrowArray* batch = &dbatch->array;
     validate_host_batch(op, batch);
@@ -762,6 +783,7 @@ b200q_status b200q_op_finish(b200q_op* op) {
   if (!op) return fail(B200Q_ERR_INVALID_ARG, "op is null");
   return guarded(op, [&] {
     if (op->finished) return;
+    require_right_side(op);
     B200Q_CUDA(cudaSetDevice(op->cx.device));
     {   // a ParquetScanExec leaf is the op's own source: read + decode the split now, one device batch per row group
       const PlanNode* leaf = op->plan.get();
@@ -792,6 +814,7 @@ b200q_status b200q_op_pull(b200q_op* op, struct ArrowArray* out, int32_t* has_ba
   if (!op || !out || !has_batch) return fail(B200Q_ERR_INVALID_ARG, "null argument");
   *has_batch = 0;
   return guarded(op, [&] {
+    if (op->taken) throw ExecError(B200Q_ERR_STATE, "pull: the op's output is the right side of a sort-merge join (b200q_op_attach_right)");
     B200Q_CUDA(cudaSetDevice(op->cx.device));
     if (!op->has_cur_host) {
       if (op->out_queue.empty()) return;
@@ -813,6 +836,7 @@ b200q_status b200q_op_pull_device(b200q_op* op, struct ArrowDeviceArray* out, in
   if (!op || !out || !has_batch) return fail(B200Q_ERR_INVALID_ARG, "null argument");
   *has_batch = 0;
   return guarded(op, [&] {
+    if (op->taken) throw ExecError(B200Q_ERR_STATE, "pull_device: the op's output is the right side of a sort-merge join (b200q_op_attach_right)");
     if (op->has_cur_host) throw ExecError(B200Q_ERR_STATE, "pull_device while a host batch is partially pulled");
     if (op->out_queue.empty()) return;
     B200Q_CUDA(cudaSetDevice(op->cx.device));
@@ -895,6 +919,25 @@ b200q_status b200q_op_attach_build(b200q_op* probe_op, b200q_op* build_op) {
     for (auto& st : probe_op->stages) if (auto* j = dynamic_cast<JoinProbeAttach*>(st.get())) a = j;
     if (!a) throw ExecError(B200Q_ERR_STATE, "attach_build: the probe op's plan has no join");
     a->attach(b->built());
+  });
+}
+
+b200q_status b200q_op_attach_right(b200q_op* join_op, b200q_op* right_op) {
+  if (!join_op || !right_op || join_op == right_op) return fail(B200Q_ERR_INVALID_ARG, "attach_right: null or identical op handles");
+  if (right_op->sticky_code) return fail(right_op->sticky_code, right_op->sticky_error);
+  return guarded(join_op, [&] {
+    SmjRightAttach* j = smj_of(join_op);
+    if (!j) throw ExecError(B200Q_ERR_STATE, "attach_right: the op's plan has no SortMergeJoinExecNode");
+    if (j->right_attached()) throw ExecError(B200Q_ERR_STATE, "attach_right: a right side is already attached");
+    if (join_op->finished || join_op->cx.m.input_batches) throw ExecError(B200Q_ERR_STATE, "attach_right: the join op already has input");
+    if (!right_op->finished) throw ExecError(B200Q_ERR_STATE, "attach_right: finish the right op first");
+    if (right_op->taken || right_op->has_cur_host || right_op->cx.m.output_batches) throw ExecError(B200Q_ERR_STATE, "attach_right: the right op's output has already been pulled or attached");
+    if (right_op->cx.device != join_op->cx.device) throw ExecError(B200Q_ERR_INVALID_ARG, "attach_right: the right op runs on another device");
+    B200Q_CUDA(cudaSetDevice(join_op->cx.device));
+    std::vector<DevBatch> batches(right_op->out_queue.begin(), right_op->out_queue.end());   // references to the device buffers: no copy
+    j->attach_right(join_op->cx, batches, right_op->out_schema);
+    right_op->out_queue.clear();
+    right_op->taken = true;
   });
 }
 

@@ -102,7 +102,7 @@ struct AggDef {
   }
 };
 
-enum NodeKind : uint8_t { N_LEAF, N_FILTER, N_PROJECT, N_AGG, N_SHUFFLE_WRITER, N_JOIN_BUILD, N_JOIN, N_SORT, N_EXPAND, N_WINDOW };
+enum NodeKind : uint8_t { N_LEAF, N_FILTER, N_PROJECT, N_AGG, N_SHUFFLE_WRITER, N_JOIN_BUILD, N_JOIN, N_SORT, N_EXPAND, N_WINDOW, N_SMJ };
 enum ShuffleKind : uint8_t { SHUFFLE_SINGLE = 0, SHUFFLE_HASH = 1, SHUFFLE_ROUND_ROBIN = 2, SHUFFLE_RANGE = 3 };   // PhysicalRepartition oneof (auron.proto:629-655)
 
 struct PlanNode {
@@ -138,6 +138,12 @@ struct PlanNode {
   std::vector<std::pair<ExprP, ExprP>> join_on;                       // (left key, right key)
   SchemaDef join_left_schema, join_right_schema;
   std::string cached_build_hash_map_id;
+  // N_SMJ (SortMergeJoinExecNode, auron.proto:432-439): `input` is the LEFT child (the op's pushed side), `smj_right` the right
+  // child (its subtree only supplies the schema: the rows come from another op, b200q_op_attach_right); join_type / join_on /
+  // join_left_schema / join_right_schema as for N_JOIN; one {asc, nulls_first} per key
+  std::shared_ptr<PlanNode> smj_right;
+  struct SortOptionsDef { bool asc = false; bool nulls_first = false; };
+  std::vector<SortOptionsDef> smj_sort_options;
   // N_LEAF, leaf_kind "ParquetScan" (ParquetScanExecNode + FileScanExecConf, auron.proto:368-419)
   struct ScanFile { std::string path; uint64_t size = 0; bool has_range = false; int64_t range_start = 0, range_end = 0; };
   std::vector<ScanFile> scan_files;
@@ -174,6 +180,10 @@ using PlanP = std::shared_ptr<PlanNode>;
 constexpr int WINDOW_MAX_EXPRS = 8;        // window expressions of one node
 constexpr int WINDOW_MAX_KEYS = 16;        // partition + order keys
 constexpr int WINDOW_MAX_COUNT_ARGS = 4;   // nullable COUNT arguments
+
+// plan_decode.cc: the key and column scope of the GPU joins (hash and sort-merge) (PlanError: UNSUPPORTED outside it, INVALID_PLAN without keys)
+void check_keys(const std::vector<ExprP>& exprs, const char* what);
+void check_data_schema(const SchemaDef& s, const char* what);
 
 // plan_decode.cc
 PlanP decode_plan(const uint8_t* bytes, size_t n, int plan_kind);

@@ -24,8 +24,6 @@ namespace {
 
 inline size_t bitmap_bytes(int64_t n) { return (size_t)((n + 31) / 32) * 4; }
 
-bool key_type_ok(const DType& t) { return t.is_integer() || t.id == T_DATE32 || t.id == T_TIMESTAMP_US; }
-
 void fill_keys(JoinKeys& k, const std::vector<ExprP>& exprs, const DevBatch& in) {
   k.nkeys = (int)exprs.size();
   for (int i = 0; i < k.nkeys; i++) {
@@ -39,24 +37,28 @@ void fill_keys(JoinKeys& k, const std::vector<ExprP>& exprs, const DevBatch& in)
   }
 }
 
-void check_keys(const std::vector<ExprP>& exprs, const char* what) {
-  if (exprs.empty()) throw PlanError(B200Q_ERR_INVALID_PLAN, std::string(what) + ": join without keys");
-  if (exprs.size() > 2) throw PlanError(B200Q_ERR_UNSUPPORTED, std::string(what) + ": more than two join keys are not on the GPU path");
-  for (auto& e : exprs) {
-    if (e->kind != E_COLUMN) throw PlanError(B200Q_ERR_UNSUPPORTED, std::string(what) + ": join key is a computed expression (project it first)");
-    if (!key_type_ok(e->type)) throw PlanError(B200Q_ERR_UNSUPPORTED, std::string(what) + ": join key of type " + e->type.str() + " is not on the GPU path");
-  }
-}
-
-void check_data_schema(const SchemaDef& s, const char* what) {
-  for (auto& f : s.fields) {
-    const int w = f.type.byte_width();
-    if (f.type.id == T_BOOL || f.type.is_varlen() || f.type.id == T_NULL || w == 0)
-      throw PlanError(B200Q_ERR_UNSUPPORTED, std::string(what) + ": a " + f.type.str() + " column in a join input is not on the GPU path");
-  }
-}
-
 }  // namespace
+
+// all columns of one side through one index vector: one kernel per 16 columns
+std::vector<DevColumn> gather_columns(OpContext& cx, const std::vector<GatherSrc>& srcs, const uint32_t* idx, int64_t n) {
+  std::vector<DevColumn> out; std::vector<DevMemP> valid_bytes;
+  for (size_t c0 = 0; c0 < srcs.size(); c0 += 16) {
+    GatherSpec g{}; g.ncols = (int)std::min<size_t>(16, srcs.size() - c0);
+    for (int c = 0; c < g.ncols; c++) {
+      const GatherSrc& s = srcs[c0 + (size_t)c];
+      DevColumn o; o.type = s.type;
+      const int w = s.type.byte_width();
+      o.values = DevMem::alloc((size_t)n * w + 16, cx.stream);
+      DevMemP ob = s.may_be_null ? DevMem::alloc((size_t)n + 16, cx.stream) : nullptr;
+      g.col[c] = GatherCol{s.values, s.vbits, s.vbytes, o.values->ptr, ob ? (uint8_t*)ob->ptr : nullptr, s.bit_offset, w};
+      out.push_back(o); valid_bytes.push_back(ob);
+    }
+    cx.m.launches += launch_join_gather_multi(g, idx, n, cx.stream);
+  }
+  for (size_t c = 0; c < out.size(); c++)
+    if (valid_bytes[c]) { out[c].validity = DevMem::alloc(bitmap_bytes(n), cx.stream, true); cx.m.launches += launch_pack_valid((const uint8_t*)valid_bytes[c]->ptr, (uint32_t*)out[c].validity->ptr, n, cx.stream); }
+  return out;
+}
 
 // ---- what a finished build op holds (shared with the probe ops that attach to it) -------------------------------------
 struct JoinBuilt {
@@ -242,27 +244,8 @@ class JoinProbeStage : public Stage, public JoinProbeAttach {
     if (!map_joined_ && (build_outer_ || (semi_like_ && !probe_is_join_side_))) map_joined_ = DevMem::alloc((size_t)built_->rows + 16, cx.stream, true);
   }
 
-  // all columns of one side through one index vector: one kernel per 16 columns
-  struct Src { DType type; const void* values; const uint8_t* vbits; uint32_t bit_offset; const uint8_t* vbytes; bool may_be_null; };
-  std::vector<DevColumn> gather_all(OpContext& cx, const std::vector<Src>& srcs, const uint32_t* idx, int64_t n) {
-    std::vector<DevColumn> out; std::vector<DevMemP> valid_bytes;
-    for (size_t c0 = 0; c0 < srcs.size(); c0 += 16) {
-      GatherSpec g{}; g.ncols = (int)std::min<size_t>(16, srcs.size() - c0);
-      for (int c = 0; c < g.ncols; c++) {
-        const Src& s = srcs[c0 + (size_t)c];
-        DevColumn o; o.type = s.type;
-        const int w = s.type.byte_width();
-        o.values = DevMem::alloc((size_t)n * w + 16, cx.stream);
-        DevMemP ob = s.may_be_null ? DevMem::alloc((size_t)n + 16, cx.stream) : nullptr;
-        g.col[c] = GatherCol{s.values, s.vbits, s.vbytes, o.values->ptr, ob ? (uint8_t*)ob->ptr : nullptr, s.bit_offset, w};
-        out.push_back(o); valid_bytes.push_back(ob);
-      }
-      cx.m.launches += launch_join_gather_multi(g, idx, n, cx.stream);
-    }
-    for (size_t c = 0; c < out.size(); c++)
-      if (valid_bytes[c]) { out[c].validity = DevMem::alloc(bitmap_bytes(n), cx.stream, true); cx.m.launches += launch_pack_valid((const uint8_t*)valid_bytes[c]->ptr, (uint32_t*)out[c].validity->ptr, n, cx.stream); }
-    return out;
-  }
+  using Src = GatherSrc;
+  std::vector<DevColumn> gather_all(OpContext& cx, const std::vector<Src>& srcs, const uint32_t* idx, int64_t n) { return gather_columns(cx, srcs, idx, n); }
   std::vector<DevColumn> gather_probe(OpContext& cx, const DevBatch& in, const uint32_t* idx, int64_t n, bool nil_possible) {
     std::vector<Src> srcs;
     for (auto& s : in.cols) {

@@ -32,25 +32,8 @@ int sgrid(int64_t n, int per_block = SB * 4) {
 __global__ void __launch_bounds__(SB) sort_normalise_kernel(const SortKeyCol k, const uint32_t* __restrict__ idx, long long n, unsigned long long* __restrict__ keys, uint8_t* __restrict__ nullrank) {
   for (long long i = blockIdx.x * (long long)SB + threadIdx.x; i < n; i += (long long)gridDim.x * SB) {
     const long long r = idx ? idx[i] : i;
-    const bool valid = k.valid_bytes ? k.valid_bytes[r] != 0 : true;
-    unsigned long long w = 0;
-    if (valid) {
-      switch (k.phys) {
-        case PH_BOOL: w = ((const uint8_t*)k.values)[r] ? 1 : 0; break;       // the stage hands Boolean keys over as bytes
-        case PH_I8: w = (uint8_t)(((const int8_t*)k.values)[r] ^ 0x80); break;
-        case PH_I16: w = (uint16_t)(((const int16_t*)k.values)[r] ^ 0x8000); break;
-        case PH_I32: w = (uint32_t)(((const int32_t*)k.values)[r]) ^ 0x80000000u; break;
-        case PH_I64: w = (unsigned long long)(((const long long*)k.values)[r]) ^ 0x8000000000000000ull; break;
-        case PH_F32: { const uint32_t b = ((const uint32_t*)k.values)[r]; w = (b & 0x80000000u) ? (uint32_t)~b : (b | 0x80000000u); break; }
-        case PH_F64: { const unsigned long long b = ((const unsigned long long*)k.values)[r]; w = (b >> 63) ? ~b : (b | 0x8000000000000000ull); break; }
-        default: {                                                         // decimal128: word 0 = low (unsigned), word 1 = high (signed)
-          const unsigned long long* p = (const unsigned long long*)k.values + 2 * r;
-          w = k.dec_word ? (p[1] ^ 0x8000000000000000ull) : p[0];
-          break;
-        }
-      }
-      if (k.descending) w = ~w & k.mask;
-    }
+    bool valid;
+    const unsigned long long w = sort_normalise_word(k, r, &valid);
     keys[i] = w;
     if (nullrank) nullrank[i] = valid ? (k.nulls_first ? 1 : 0) : (k.nulls_first ? 0 : 1);
   }

@@ -837,6 +837,57 @@ PlanP parse_join(Reader r, bool broadcast) {
   return n;
 }
 
+// SortMergeJoinExecNode{schema=1, left=2, right=3, on=4, sort_options=5{asc=1, nulls_first=2}, join_type=6} (from_proto.rs:224-262),
+// validated like SortMergeJoinExec::create_join_params (sort_merge_join_exec.rs:90-130) and, for the GPU path, like the hash join
+PlanP parse_smj(Reader r) {
+  auto n = std::make_shared<PlanNode>(); n->kind = N_SMJ;
+  PlanP left, right; std::vector<Reader> on; bool have_schema = false;
+  while (!r.done()) {
+    int wt; uint32_t f = r.tag(wt);
+    switch (f) {
+      case 1: n->schema = parse_schema(r.bytes()); have_schema = true; break;
+      case 2: left = parse_plan(r.bytes()); break;
+      case 3: right = parse_plan(r.bytes()); break;
+      case 4: on.push_back(r.bytes()); break;
+      case 5: {
+        Reader so = r.bytes(); PlanNode::SortOptionsDef d;
+        while (!so.done()) { int w2; uint32_t g = so.tag(w2); if (g == 1) d.asc = so.varint() != 0; else if (g == 2) d.nulls_first = so.varint() != 0; else so.skip(w2); }
+        n->smj_sort_options.push_back(d); break;
+      }
+      case 6: n->join_type = (int)r.varint(); break;
+      default: r.skip(wt);
+    }
+  }
+  if (!have_schema || !left || !right) bad("Missing required field in protobuf");
+  if (n->join_type < 0 || n->join_type > 6) bad("invalid JoinType");
+  n->join_left_schema = left->schema; n->join_right_schema = right->schema;
+  std::vector<ExprP> lk, rk;
+  for (auto& o : on) {                         // JoinOn{left=1, right=2}
+    Reader jr = o; ExprP l, rr;
+    while (!jr.done()) { int wt; uint32_t f = jr.tag(wt); if (f == 1) l = parse_expr(jr.bytes(), n->join_left_schema); else if (f == 2) rr = parse_expr(jr.bytes(), n->join_right_schema); else jr.skip(wt); }
+    if (!l || !rr) bad("JoinOn without both sides");
+    n->join_on.push_back({l, rr}); lk.push_back(l); rk.push_back(rr);
+  }
+  if (n->smj_sort_options.size() != n->join_on.size())
+    bad("SortMergeJoinExec: " + std::to_string(n->smj_sort_options.size()) + " sort_options for " + std::to_string(n->join_on.size()) + " join keys");
+  for (auto& p : n->join_on)
+    if (p.first->type != p.second->type) bad("join key data type differs " + p.first->type.str() + " <-> " + p.second->type.str());
+  check_keys(lk, "SortMergeJoinExec"); check_keys(rk, "SortMergeJoinExec");
+  check_data_schema(n->join_left_schema, "SortMergeJoinExec"); check_data_schema(n->join_right_schema, "SortMergeJoinExec");
+  // output = left ++ right, left for LeftSemi / LeftAnti, left ++ Boolean for Existence (as the hash join's probe stage checks it)
+  const bool semi_like = n->join_type >= 4;
+  const size_t nl = n->join_left_schema.fields.size();
+  const size_t want = n->join_type == 6 ? nl + 1 : (semi_like ? nl : nl + n->join_right_schema.fields.size());
+  if (n->schema.fields.size() != want) bad("join schema has " + std::to_string(n->schema.fields.size()) + " fields, the join produces " + std::to_string(want));
+  for (size_t i = 0; i < want; i++) {
+    const DType& got = n->schema.fields[i].type;
+    DType exp; if (i < nl) exp = n->join_left_schema.fields[i].type; else if (n->join_type == 6) exp.id = T_BOOL; else exp = n->join_right_schema.fields[i - nl].type;
+    if (got != exp) bad("join schema field " + std::to_string(i) + " is " + got.str() + ", the inputs give " + exp.str());
+  }
+  n->input = left; n->smj_right = right;
+  return n;
+}
+
 PlanP parse_plan(Reader r) {                  // PhysicalPlanNode oneof (auron.proto:27-55)
   while (!r.done()) {
     int wt; uint32_t f = r.tag(wt);
@@ -855,7 +906,8 @@ PlanP parse_plan(Reader r) {                  // PhysicalPlanNode oneof (auron.p
       case 18: return parse_leaf(r.bytes(), true);
       case 20: return parse_expand(r.bytes());
       case 22: return parse_window(r.bytes());
-      case 1: case 4: case 9: case 10: case 14: case 17: case 19:
+      case 10: return parse_smj(r.bytes());
+      case 1: case 4: case 9: case 14: case 17: case 19:
       case 21: case 23: case 24: case 25:
         unsupported("plan node #" + std::to_string(f) + " is outside the Filter/Project/Agg hot path (SURVEY.md §8)");
       default: r.skip(wt);
@@ -870,6 +922,25 @@ const char* binop_name(BinOp op) {
 }
 
 }  // namespace
+
+static bool key_type_ok(const DType& t) { return t.is_integer() || t.id == T_DATE32 || t.id == T_TIMESTAMP_US; }
+
+void check_keys(const std::vector<ExprP>& exprs, const char* what) {
+  if (exprs.empty()) throw PlanError(B200Q_ERR_INVALID_PLAN, std::string(what) + ": join without keys");
+  if (exprs.size() > 2) throw PlanError(B200Q_ERR_UNSUPPORTED, std::string(what) + ": more than two join keys are not on the GPU path");
+  for (auto& e : exprs) {
+    if (e->kind != E_COLUMN) throw PlanError(B200Q_ERR_UNSUPPORTED, std::string(what) + ": join key is a computed expression (project it first)");
+    if (!key_type_ok(e->type)) throw PlanError(B200Q_ERR_UNSUPPORTED, std::string(what) + ": join key of type " + e->type.str() + " is not on the GPU path");
+  }
+}
+
+void check_data_schema(const SchemaDef& s, const char* what) {
+  for (auto& f : s.fields) {
+    const int w = f.type.byte_width();
+    if (f.type.id == T_BOOL || f.type.is_varlen() || f.type.id == T_NULL || w == 0)
+      throw PlanError(B200Q_ERR_UNSUPPORTED, std::string(what) + ": a " + f.type.str() + " column in a join input is not on the GPU path");
+  }
+}
 
 std::string explain_expr(const ExprP& e) {
   std::ostringstream o;
@@ -984,6 +1055,17 @@ static void explain_rec(const PlanP& p, int depth, std::ostringstream& o) {
       o << "] map_side=" << (p->join_build_is_left ? "Left" : "Right") << " schema=" << schema_str(p->schema) << "\n";
       o << ind << "  [map side]\n"; explain_rec(p->join_build, depth + 2, o);
       o << ind << "  [probed side]\n"; explain_rec(p->input, depth + 2, o);
+      return;
+    }
+    case N_SMJ: {
+      static const char* jt[] = {"Inner", "Left", "Right", "Full", "LeftSemi", "LeftAnti", "Existence"};
+      o << ind << "SortMergeJoin: join_type=" << jt[p->join_type] << ", on=[";
+      for (size_t i = 0; i < p->join_on.size(); i++) o << (i ? ", " : "") << "(" << explain_expr(p->join_on[i].first) << ", " << explain_expr(p->join_on[i].second) << ")";
+      o << "], sort_options=[";
+      for (size_t i = 0; i < p->smj_sort_options.size(); i++) o << (i ? ", " : "") << (p->smj_sort_options[i].asc ? "ASC" : "DESC") << (p->smj_sort_options[i].nulls_first ? " NULLS FIRST" : " NULLS LAST");
+      o << "] schema=" << schema_str(p->schema) << "\n";
+      o << ind << "  [left]\n"; explain_rec(p->input, depth + 2, o);
+      o << ind << "  [right]\n"; explain_rec(p->smj_right, depth + 2, o);
       return;
     }
     case N_SHUFFLE_WRITER: {

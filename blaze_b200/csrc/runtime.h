@@ -148,8 +148,22 @@ std::unique_ptr<Stage> make_window_stage(OpContext& cx, const SchemaDef& in_sche
 struct JoinBuilt;
 std::unique_ptr<Stage> make_join_build_stage(OpContext& cx, const SchemaDef& in_schema, const PlanNode& node);
 std::unique_ptr<Stage> make_join_probe_stage(OpContext& cx, const SchemaDef& in_schema, const PlanNode& node);
+// all `srcs` through one index vector (JOIN_NIL: a NULL row): one gather kernel per 16 columns (join_stage.cu).  A source's
+// validity is vbytes (one byte per row), else vbits at bit_offset, else none; may_be_null: the output gets a validity bitmap
+struct GatherSrc { DType type; const void* values; const uint8_t* vbits; uint32_t bit_offset; const uint8_t* vbytes; bool may_be_null; };
+std::vector<DevColumn> gather_columns(OpContext& cx, const std::vector<GatherSrc>& srcs, const uint32_t* idx, int64_t n);
 struct JoinBuildResult { virtual ~JoinBuildResult() {} virtual std::shared_ptr<JoinBuilt> built() const = 0; };
 struct JoinProbeAttach { virtual ~JoinProbeAttach() {} virtual void attach(std::shared_ptr<JoinBuilt> b) = 0; };
+
+// SortMergeJoinExec (smj_stage.cu): the op's pushed input is the LEFT side; the right side is the queued output of another,
+// finished op (b200q_op_attach_right), taken over by reference at attach
+std::unique_ptr<Stage> make_smj_stage(OpContext& cx, const SchemaDef& in_schema, const PlanNode& node);
+struct SmjRightAttach {
+  virtual ~SmjRightAttach() {}
+  virtual bool right_attached() const = 0;
+  // `schema`: the right op's output schema; throws ExecError (INVALID_ARG: schema, unsorted; UNSUPPORTED: 2^31 rows or more)
+  virtual void attach_right(OpContext& cx, const std::vector<DevBatch>& batches, const SchemaDef& schema) = 0;
+};
 
 // a column as the kernels see it (stages.cu)
 DevCol dev_col_of(const DevColumn& c);

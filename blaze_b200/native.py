@@ -76,7 +76,7 @@ SYMBOLS = ["b200q_version", "b200q_build_info", "b200q_last_error", "b200q_devic
            "b200q_plan_explain", "b200q_op_create", "b200q_op_input_schema", "b200q_op_output_schema", "b200q_op_push",
            "b200q_op_push_device", "b200q_op_finish", "b200q_op_pull", "b200q_op_pull_device", "b200q_op_sync",
            "b200q_op_metrics", "b200q_op_destroy", "b200q_murmur3_partition",
-           "b200q_set_file_reader", "b200q_parquet_explain", "b200q_snappy_uncompress", "b200q_op_attach_build", "b200q_op_shuffle_chunk_count", "b200q_op_shuffle_chunk", "b200q_lz4_frame_compress",
+           "b200q_set_file_reader", "b200q_parquet_explain", "b200q_snappy_uncompress", "b200q_op_attach_build", "b200q_op_attach_right", "b200q_op_shuffle_chunk_count", "b200q_op_shuffle_chunk", "b200q_lz4_frame_compress",
            "b200q_lz4_frame_decompress", "b200q_op_push_ipc",
            "b200q_exchange_unique_id", "b200q_exchange_create", "b200q_exchange_shuffle", "b200q_exchange_kernel_launches",
            "b200q_exchange_destroy"]
@@ -110,6 +110,7 @@ def _load():
     lib.b200q_parquet_explain.argtypes = [C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.b200q_snappy_uncompress.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.b200q_op_attach_build.argtypes = [C.c_void_p, C.c_void_p]
+    lib.b200q_op_attach_right.argtypes = [C.c_void_p, C.c_void_p]
     lib.b200q_op_shuffle_chunk_count.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
     lib.b200q_op_shuffle_chunk.argtypes = [C.c_void_p, C.c_int64, C.POINTER(ShuffleChunk)]
     lib.b200q_lz4_frame_compress.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -327,6 +328,10 @@ class NativeOp:
     def attach_build(self, build_op: "NativeOp"):
         """join ops: use the finished map side held by `build_op` (a BroadcastJoinBuildHashMapExecNode op)"""
         check(lib.b200q_op_attach_build(self._h, build_op._h))
+
+    def attach_right(self, right_op: "NativeOp"):
+        """sort-merge join ops: take the queued output of `right_op` (finished, not pulled) as the join's right side"""
+        check(lib.b200q_op_attach_right(self._h, right_op._h))
 
     def shuffle_chunks(self) -> List[dict]:
         """ShuffleWriterExec plans, after finish(): [{rows, part_off, part_rows, data (bytes, host) | data_ptr (device)}]"""

@@ -57,9 +57,21 @@ class ExecutionPlan:
         native.plan_explain(self.plan_bytes())
 
     def execute(self, conf: Optional[native.Conf] = None, device: int = 0):
-        """Run the subtree on the GPU over the leaf's batches; yields pyarrow RecordBatches."""
+        """Run the subtree on the GPU over the leaf's batches; yields pyarrow RecordBatches.  A SortMergeJoinExec on the way to the
+        leaf gets its right side first: that subtree runs as its own op, which is finished and attached to this one."""
         leaf = self.leaf()
+        smj = self
+        while smj.children() and not isinstance(smj, SortMergeJoinExec):
+            smj = smj.children()[0]
         with native.NativeOp(self.plan_bytes(), conf, device) as op:
+            if isinstance(smj, SortMergeJoinExec):
+                with native.NativeOp(smj.right.plan_bytes(), conf, device) as rop:
+                    rleaf = smj.right.leaf()
+                    for rb in rleaf.batches:
+                        rleaf.push_to(rop, rb)
+                    rop.finish()
+                    smj.right_metrics = rop.metrics()
+                    op.attach_right(rop)
             for rb in leaf.batches:
                 leaf.push_to(op, rb)
                 while True:
@@ -382,6 +394,30 @@ class BroadcastJoinExec(ExecutionPlan):
                 op.finish()
                 yield from op.pull_all()
                 self.last_metrics = op.metrics()
+
+
+class SortMergeJoinExec(ExecutionPlan):
+    """SortMergeJoinExec::try_new(schema, left, right, on, join_type, sort_options) (sort_merge_join_exec.rs:71-90): an equi-join of two
+    inputs each sorted by its keys; sort_options = [(asc, nulls_first)], one per key (arrow SortOptions{descending = !asc}).
+    execute(): the right subtree runs as its own op, is finished and attached (b200q_op_attach_right), then the left side is pushed
+    (ExecutionPlan.execute, also when the join sits below other operators of the same op)."""
+
+    def __init__(self, schema: Schema, left: ExecutionPlan, right: ExecutionPlan, on, sort_options, join_type: int):
+        self._schema, self.left, self.right, self.on = schema, left, right, list(on)
+        self.sort_options = [(bool(a), bool(nf)) for a, nf in sort_options]
+        self.join_type = join_type
+        self._validate()
+
+    try_new = classmethod(lambda cls, *a, **k: cls(*a, **k))
+
+    def schema(self):
+        return self._schema
+
+    def children(self):
+        return [self.left, self.right]
+
+    def node(self):
+        return P.smj_node(self._schema, self.left.node(), self.right.node(), self.on, self.sort_options, self.join_type)
 
 
 class ShuffleWriterExec(ExecutionPlan):

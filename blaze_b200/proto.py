@@ -179,6 +179,7 @@ def _build_pool():
         ("empty_partitions", 15, "EmptyPartitionsExecNode", O), ("agg", 16, "AggExecNode", O),
         ("ffi_reader", 18, "FFIReaderExecNode", O), ("expand", 20, "PhysicalPlanNode.ExpandExecNode", O),
         ("window", 22, "PhysicalPlanNode.WindowExecNode", O), ("ipc_reader", 3, "PhysicalPlanNode.IpcReaderExecNode", O),
+        ("sort_merge_join", 10, "PhysicalPlanNode.SortMergeJoinExecNode", O),
     ], oneofs=["PhysicalPlanType"])
     # ExpandExecNode{input=1, schema=2, projections=3} and ExpandProjection{expr=1} (auron.proto:714-722) are top-level in the reference;
     # nested here like the string-match nodes above (same bytes on the wire), the top-level set stays that of the field table of
@@ -207,6 +208,11 @@ def _build_pool():
     # tests/golden/auron_proto_ipc_reader_fields.json
     _msg(fd, "IpcReaderExecNode", [("num_partitions", 1, _F.TYPE_UINT32), ("schema", 2, "Schema"), ("ipc_provider_resource_id", 3, _F.TYPE_STRING)],
          into=pp.nested_type)
+    # SortMergeJoinExecNode and SortOptions (auron.proto:432-439, 485-488): nested the same way; tests/test_proto_smj_compat.py checks
+    # them against tests/golden/auron_proto_smj_fields.json
+    _msg(fd, "SortMergeJoinExecNode", [("schema", 1, "Schema"), ("left", 2, "PhysicalPlanNode"), ("right", 3, "PhysicalPlanNode"), ("on", 4, "JoinOn", R),
+                                       ("sort_options", 5, "PhysicalPlanNode.SortOptions", R), ("join_type", 6, "enum:JoinType")], into=pp.nested_type)
+    _msg(fd, "SortOptions", [("asc", 1, _F.TYPE_BOOL), ("nulls_first", 2, _F.TYPE_BOOL)], into=pp.nested_type)
     _msg(fd, "PartitionId", [("stage_id", 2, _F.TYPE_UINT32), ("partition_id", 4, _F.TYPE_UINT32), ("task_id", 5, _F.TYPE_UINT64)])
     _msg(fd, "TaskDefinition", [("task_id", 1, "PartitionId"), ("plan", 2, "PhysicalPlanNode")])
 
@@ -514,6 +520,24 @@ def join_node(schema: Schema, left_node, right_node, on, join_type: int, map_sid
         j.cached_build_hash_map_id = cached_id
     else:
         j.build_side = map_side
+    return n
+
+
+def smj_node(schema: Schema, left_node, right_node, on, sort_options, join_type: int):
+    """SortMergeJoinExecNode; on = [(left expr, right expr)], sort_options = [(asc, nulls_first)] (one per key)"""
+    n = PhysicalPlanNode()
+    j = n.sort_merge_join
+    j.schema.CopyFrom(schema_msg(schema))
+    j.left.CopyFrom(left_node)
+    j.right.CopyFrom(right_node)
+    for l, r in on:
+        o = j.on.add()
+        o.left.CopyFrom(expr_msg(l))
+        o.right.CopyFrom(expr_msg(r))
+    for asc, nulls_first in sort_options:
+        x = j.sort_options.add()
+        x.asc, x.nulls_first = asc, nulls_first
+    j.join_type = join_type
     return n
 
 

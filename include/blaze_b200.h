@@ -39,6 +39,7 @@
  *   ParquetScanExecNode leaf ParquetExec::execute (decode + row-group pruning)      datafusion-ext-plans/src/parquet_exec.rs:150-203,316-396
  *   SortExecNode plans      SortExec::new + ExternalSorter::insert_batch / output   datafusion-ext-plans/src/sort_exec.rs:97-112,626-752
  *   b200q_op_attach_build   collect_join_hash_map + execute_join_with_map   datafusion-ext-plans/src/broadcast_join_exec.rs:317-385,562-639
+ *   b200q_op_attach_right   SortMergeJoinExec::execute (the right child's stream)   datafusion-ext-plans/src/sort_merge_join_exec.rs:200-330
  *   b200q_op_push_ipc       IpcReaderExec::execute (decode of the shuffle blocks)  datafusion-ext-plans/src/ipc_reader_exec.rs:164-272
  *   b200q_op_shuffle_chunk  the per-partition encoded bytes before compression — what BufferedData::write_rss
  *                           hands to an RSS partition writer (buffered_data.rs:160-196)
@@ -137,7 +138,8 @@ typedef struct b200q_conf {
                                          rows before one H2D + one kernel launch (default 1<<20)  */
   int64_t agg_initial_groups;         /* initial hash-table sizing hint in groups (default 1<<19) */
   int64_t max_launch_rows;            /* rows per kernel launch for device-resident pushes
-                                         (default 1<<27)                                          */
+                                         (default 1<<27); a sort-merge join also emits its output
+                                         in batches of at most this many rows                     */
   int32_t partial_state_columnar;     /* 1: non-final agg output/input uses typed state columns
                                          (GPU-to-GPU exchange) instead of the reference's Binary
                                          frozen-row column `#9223372036854775807`                 */
@@ -238,6 +240,22 @@ void b200q_op_destroy(b200q_op* op);
  * cached_build_hash_map_id (broadcast_join_exec.rs:640-677); the build op must outlive them only until they are destroyed
  * (the table is reference counted).  Inner / Left / Right / Full / LeftSemi / LeftAnti / Existence, either side as the map. */
 b200q_status b200q_op_attach_build(b200q_op* probe_op, b200q_op* build_op);
+
+/* ---- sort-merge join: the right side (plans with a SortMergeJoinExecNode) -------------------------------------------------
+ * Reference: SortMergeJoinExec (datafusion-ext-plans/src/sort_merge_join_exec.rs, joins/smj).  The op created from the
+ * SortMergeJoinExecNode subtree takes its LEFT child as its pushed input (push / push_device / push_ipc; stages below the join,
+ * typically a SortExec, run in the same op).  `right_op` is an op built from the node's RIGHT child subtree (e.g. IpcReader ->
+ * SortExec), finished and not yet pulled: its queued device batches become the join's right side by reference, without a copy
+ * when there is one batch (several are concatenated once).  Afterwards b200q_op_pull / pull_device on `right_op` is
+ * B200Q_ERR_STATE, and `right_op` may be destroyed (the batches are reference counted).  Status: B200Q_ERR_INVALID_ARG when the
+ * right op's output schema differs from the node's right schema, or the right rows are not sorted by the join keys under the
+ * node's sort_options; B200Q_ERR_STATE when `right_op` is unfinished or already pulled / attached, when the join op already has
+ * a right side or input, and for any push or finish on the join op before this call; B200Q_ERR_UNSUPPORTED for 2^31 right rows
+ * or more.  Each side must arrive sorted by its keys: the op checks every left batch, across batch boundaries, and refuses it
+ * (B200Q_ERR_INVALID_ARG) instead of returning wrong rows.  Inner / Left / LeftSemi / LeftAnti / Existence output follows the left
+ * input order (a left row's rows are contiguous, its matches in right order); Right follows the right keys' order; Full is
+ * merged the same way; on equal keys, left-driven rows come before right-only rows. */
+b200q_status b200q_op_attach_right(b200q_op* join_op, b200q_op* right_op);
 
 /* ---- ParquetScanExec as the source of an op (plans whose leaf is a ParquetScanExecNode) -----------------------------------
  * Reference: ParquetExec::execute (datafusion-ext-plans/src/parquet_exec.rs:150-203) + the FsProvider byte-range reads

@@ -772,3 +772,75 @@ if any(t in (ONLY or "R1,R2") for t in ("R1", "R2")):
                           "launches": m["gpu_kernel_launches"], "elapsed_compute_ms": m["elapsed_compute_ns"] / 1e6}), flush=True)
     import shutil
     shutil.rmtree(tmp, ignore_errors=True)
+
+
+# MJ1-MJ2: SortMergeJoinExec (DESIGN §3.14), store_sales ⋈ store_returns on (item_sk, ticket_number): a left side of 2^26 rows against a
+# right side of 2^24 rows, two int64 keys, four int64 payload columns per side, about 10 % of the left rows matching; Inner and Left.
+# MJ1: both sides device-resident and already sorted; MJ2: the same rows shuffled, with a SortExec below the join in each op.  Timed
+# whole-op: from the right op's push_device to the join op's sync, right op, attach and pulls of the output (device) included.
+# alg bytes = keys + payload read once per side (48 B/row) + the output written (96 B/row).  The output count is checked against a
+# torch searchsorted count of the same keys.
+def _wanted(shape):                                # SHAPES tokens are substrings of the shape names, as in run()
+    return not ONLY or any(t in shape for t in ONLY.split(","))
+
+
+if _wanted("MJ1") or _wanted("MJ2"):
+    import subprocess, time
+    card = torch.cuda.get_device_name(0)
+    try:
+        plim = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True).stdout.strip()
+    except OSError:
+        plim = "unknown"
+    nl, nr = int(os.environ.get("MJ_LEFT", 1 << 26)), int(os.environ.get("MJ_RIGHT", 1 << 24))
+    item = torch.randint(0, 1 << 18, (nl,), dtype=torch.int64, device=dev, generator=g)
+    ticket = torch.randint(0, 1 << 30, (nl,), dtype=torch.int64, device=dev, generator=g)
+    pick = torch.randperm(nl, device=dev, generator=g)[:nr]
+    fresh = torch.rand(nr, device=dev, generator=g) < 0.6                        # returns of sales this side does not hold: never match
+    r_item = item[pick].clone()
+    r_ticket = torch.where(fresh, torch.randint(1 << 30, 1 << 31, (nr,), dtype=torch.int64, device=dev, generator=g), ticket[pick])
+    def sides(sort):
+        li, lt, ri, rt = item, ticket, r_item, r_ticket
+        if sort:
+            o = torch.argsort(li * (1 << 31) + lt, stable=True); li, lt = li[o], lt[o]
+            o = torch.argsort(ri * (1 << 31) + rt, stable=True); ri, rt = ri[o], rt[o]
+        lp = [torch.randint(-2**62, 2**62, (nl,), dtype=torch.int64, device=dev, generator=g) for _ in range(4)]
+        rp = [torch.randint(-2**62, 2**62, (nr,), dtype=torch.int64, device=dev, generator=g) for _ in range(4)]
+        return [li.contiguous(), lt.contiguous()] + lp, [ri.contiguous(), rt.contiguous()] + rp
+    lkey, rkey = item * (1 << 31) + ticket, torch.sort(r_item * (1 << 31) + r_ticket).values
+    per_left = torch.searchsorted(rkey, lkey, right=True) - torch.searchsorted(rkey, lkey)
+    expect = {PL.JOIN_INNER: int(per_left.sum()), PL.JOIN_LEFT: int(per_left.clamp(min=1).sum())}
+    ls = T.Schema([T.Field("item", T.int64, False), T.Field("ticket", T.int64, False)] + [T.Field(f"l{i}", T.int64, False) for i in range(4)])
+    rs = T.Schema([T.Field("r_item", T.int64, False), T.Field("r_ticket", T.int64, False)] + [T.Field(f"r{i}", T.int64, False) for i in range(4)])
+    on = [(E.Column("item"), E.Column("r_item")), (E.Column("ticket"), E.Column("r_ticket"))]
+    for shape, presorted in (("MJ1", True), ("MJ2", False)):
+        if not _wanted(shape): continue
+        lcols, rcols = sides(presorted)
+        for jt, jname in ((PL.JOIN_INNER, "Inner"), (PL.JOIN_LEFT, "Left")):
+            left, right = PL.MemoryExec(ls), PL.MemoryExec(rs)
+            if not presorted:
+                left = PL.SortExec(left, [(E.Column("item"), False, True), (E.Column("ticket"), False, True)])
+                right = PL.SortExec(right, [(E.Column("r_item"), False, True), (E.Column("r_ticket"), False, True)])
+            plan = PL.SortMergeJoinExec(PL.build_join_schema(ls, rs, jt), left, right, on, [(True, True), (True, True)], jt)
+            best = None
+            for _ in range(REPS or 3):
+                with native.NativeOp(plan.plan_bytes(), None, 0) as op, native.NativeOp(right.plan_bytes(), None, 0) as rop:
+                    torch.cuda.synchronize(); t0 = time.perf_counter()
+                    rop.push_device(native.DeviceBatch([(c.data_ptr(), 0, nr) for c in rcols], nr, 0, keepalive=rcols)); rop.finish()
+                    op.attach_right(rop)
+                    op.push_device(native.DeviceBatch([(c.data_ptr(), 0, nl) for c in lcols], nl, 0, keepalive=lcols)); op.finish()
+                    n_out = 0
+                    while True:
+                        o = op.pull_device()
+                        if o is None: break
+                        n_out += o.array.length; native.release_device_array(o)
+                    op.sync()
+                    dt = time.perf_counter() - t0
+                    m = op.metrics()
+                if best is None or dt < best[0]: best = (dt, n_out, m)
+            dt, n_out, m = best
+            alg = 48.0 * (nl + nr) + 96.0 * n_out
+            print(json.dumps({"shape": f"{shape} {jname} SMJ (item, ticket) {nl} x {nr} rows" + (" pre-sorted" if presorted else " with SortExec in both ops"),
+                              "card": card, "power_limit": plim, "out_rows": n_out, "verified_rows": n_out == expect[jt], "wall_ms_push_to_sync": dt * 1e3,
+                              "left_rows_per_s": nl / dt, "alg_GBps": alg / dt / 1e9, "frac_of_hbm_peak": alg / dt / 1e9 / peak,
+                              "launches": m["gpu_kernel_launches"]}), flush=True)
+        del lcols, rcols
