@@ -14,6 +14,9 @@ namespace b200q {
 typedef __int128 i128;
 
 static i128 pow10_i128(int n) { i128 v = 1; for (int i = 0; i < n; i++) v *= 10; return v; }
+// 10^n as the correctly rounded f64 (i128 -> double rounds once).  libm's pow need not be: glibc 2.39 returns 10^23 one ulp
+// high, so the decimal <-> float casts of scale 23 would depend on the host's libm.
+static double pow10_f64(int n) { return (double)pow10_i128(n); }
 
 PhysKind phys_of(const DType& t) {
   switch (t.id) {
@@ -178,10 +181,10 @@ struct Compiler {
       emit(VM_CAST_DEC_I, (uint8_t)to.int_bits(), 0, pool({lo(f), hi(f)})); pop(2); push(1); return 1;
     }
     if (from.is_decimal() && to.is_float()) {
-      emit(VM_CAST_DEC_F, to.id == T_FLOAT32, 0, pool({dbits(std::pow(10.0, from.scale))})); pop(2); push(1); return 1;
+      emit(VM_CAST_DEC_F, to.id == T_FLOAT32, 0, pool({dbits(pow10_f64(from.scale))})); pop(2); push(1); return 1;
     }
     if (from.is_float() && to.is_decimal()) {
-      emit(VM_CAST_F_DEC, 0, 0, pool({dbits(std::pow(10.0, to.scale)), lo(lim), hi(lim)})); pop(1); push(2); return 2;
+      emit(VM_CAST_F_DEC, 0, 0, pool({dbits(pow10_f64(to.scale)), lo(lim), hi(lim)})); pop(1); push(2); return 2;
     }
     throw PlanError(B200Q_ERR_UNSUPPORTED, "cast " + from.str() + " -> " + to.str() + " is not on the hot path");
   }

@@ -444,7 +444,8 @@ __device__ __forceinline__ int vm_run(const VmInstr* __restrict__ code, const ui
             if (in.a == 1) {
               const i128_t dropped = v % f; v = v / f;
               const i128_t ad = dropped < 0 ? -dropped : dropped;
-              if (ad * 2 >= f) v += dropped < 0 ? -1 : 1;
+              // release build: `dropped.abs() * 2` wraps, so |dropped| >= 2^126 (a 38-digit scale drop) does not round
+              if ((i128_t)((u128_t)ad * 2) >= f) v += dropped < 0 ? -1 : 1;
             } else if (in.a == 2) v = (i128_t)((u128_t)v * (u128_t)f);       // release build: wrapping multiply
             ok = !(v <= -lim || v >= lim);
           }

@@ -25,6 +25,7 @@ from __future__ import annotations
 import math
 import struct
 from dataclasses import dataclass
+from fractions import Fraction
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -416,7 +417,7 @@ def _change_precision(v: int, precision: int, scale: int, to_p: int, to_s: int) 
         q, rem = divmod(abs(v), p10)
         v = -q if neg else q                         # Rust `/` and `%` round toward zero
         dropped = -rem if neg else rem
-        if abs(dropped) * 2 >= p10:
+        if wrap_i128(abs(dropped) * 2) >= p10:         # release build: the i128 product wraps (no rounding for |dropped| >= 2^126)
             v += -1 if dropped < 0 else 1
     elif to_s > scale:
         v = wrap_i128(v * 10 ** (to_s - scale))      # release build: wrapping multiply
@@ -580,7 +581,8 @@ def cast(c: Col, to: DataType) -> Col:
         for i in range(n):
             f = float(c.values[i]) * mul
             if valid[i] and math.isfinite(f):
-                r = int(math.floor(abs(f) + 0.5))                        # f64::round: half away from zero
+                q = Fraction(f)                                          # f64::round: half away from zero, exactly
+                r = math.floor(abs(q) + Fraction(1, 2))                  # (floor(|f| + 0.5) in f64 rounds the sum first)
                 r = -r if f < 0 else r
                 if -lim < r < lim:
                     vals[i] = r
