@@ -22,8 +22,6 @@ namespace b200q {
 
 namespace {
 
-inline size_t bitmap_bytes(int64_t n) { return (size_t)((n + 31) / 32) * 4; }
-
 void fill_keys(JoinKeys& k, const std::vector<ExprP>& exprs, const DevBatch& in) {
   k.nkeys = (int)exprs.size();
   for (int i = 0; i < k.nkeys; i++) {
@@ -56,7 +54,7 @@ std::vector<DevColumn> gather_columns(OpContext& cx, const std::vector<GatherSrc
     cx.m.launches += launch_join_gather_multi(g, idx, n, cx.stream);
   }
   for (size_t c = 0; c < out.size(); c++)
-    if (valid_bytes[c]) { out[c].validity = DevMem::alloc(bitmap_bytes(n), cx.stream, true); cx.m.launches += launch_pack_valid((const uint8_t*)valid_bytes[c]->ptr, (uint32_t*)out[c].validity->ptr, n, cx.stream); }
+    if (valid_bytes[c]) out[c].validity = pack_bits(cx, valid_bytes[c]->ptr, n);
   return out;
 }
 
@@ -64,9 +62,7 @@ std::vector<DevColumn> gather_columns(OpContext& cx, const std::vector<GatherSrc
 struct JoinBuilt {
   SchemaDef schema;                               // the side's data schema
   std::vector<DType> key_types;
-  int64_t rows = 0;
-  std::vector<DevMemP> values;                    // per column, contiguous
-  std::vector<DevMemP> valid_bytes;               // per column: one byte per row, null when the column has no NULL
+  ByteCols cols;                                  // the side's rows
   JoinTable table{};
   DevMemP t_keys, t_state, t_head, t_count, t_next, t_stats, t_packed;
   uint32_t max_dup = 0;                           // rows of the most duplicated key
@@ -77,7 +73,7 @@ namespace {
 
 class JoinBuildStage : public Stage, public JoinBuildResult {
   std::vector<ExprP> keys_;
-  std::vector<DevBatch> parts_;                   // owned copies of the pushed batches
+  std::vector<ByteCols> parts_;                   // owned copies of the pushed batches
   std::shared_ptr<JoinBuilt> built_;
 
  public:
@@ -92,21 +88,8 @@ class JoinBuildStage : public Stage, public JoinBuildResult {
 
   void push(OpContext& cx, DevBatch& in, std::vector<DevBatch>&) override {
     if (built_) throw ExecError(B200Q_ERR_STATE, "join build side: push after finish");
-    const int64_t n = in.num_rows;
-    if (n == 0) return;
-    DevBatch own; own.num_rows = n;
-    for (auto& c : in.cols) {                     // the caller's buffers are released when push returns: keep an owned copy
-      DevColumn o; o.type = c.type;
-      const size_t w = (size_t)c.type.byte_width();
-      o.values = DevMem::alloc((size_t)n * w, cx.stream);
-      B200Q_CUDA(cudaMemcpyAsync(o.values->ptr, (const uint8_t*)c.values->ptr + (size_t)c.offset * w, (size_t)n * w, cudaMemcpyDeviceToDevice, cx.stream));
-      if (c.validity) {                           // as one byte per row
-        o.validity = DevMem::alloc((size_t)n, cx.stream);
-        cx.m.launches += launch_unpack_bits((const uint8_t*)c.validity->ptr, (uint32_t)c.offset, n, (uint8_t*)o.validity->ptr, cx.stream);
-      }
-      own.cols.push_back(o);
-    }
-    parts_.push_back(std::move(own));
+    if (in.num_rows == 0) return;
+    parts_.push_back(to_byte_cols(cx, in_schema, {&in}));         // the caller's buffers are released when push returns: keep an owned copy
   }
 
   void finish(OpContext& cx, std::vector<DevBatch>&) override {
@@ -115,28 +98,9 @@ class JoinBuildStage : public Stage, public JoinBuildResult {
     b->schema = in_schema; b->device = cx.device;
     for (auto& e : keys_) b->key_types.push_back(e->type);
     int64_t total = 0;
-    for (auto& p : parts_) total += p.num_rows;
+    for (auto& p : parts_) total += p.rows;
     if (total >= (1LL << 30)) throw ExecError(B200Q_ERR_UNSUPPORTED, "join hash table: number of rows exceeded 2^30");     // join_hash_map.rs:107-110
-    b->rows = total;
-    const size_t ncols = in_schema.fields.size();
-    b->values.resize(ncols); b->valid_bytes.resize(ncols);
-    for (size_t c = 0; c < ncols; c++) {
-      const size_t w = (size_t)in_schema.fields[c].type.byte_width();
-      b->values[c] = DevMem::alloc((size_t)total * w + 16, cx.stream);
-      bool any_valid = false;
-      for (auto& p : parts_) any_valid = any_valid || p.cols[c].validity;
-      if (any_valid) b->valid_bytes[c] = DevMem::alloc((size_t)total + 16, cx.stream);
-      int64_t at = 0;
-      for (auto& p : parts_) {
-        B200Q_CUDA(cudaMemcpyAsync((uint8_t*)b->values[c]->ptr + (size_t)at * w, p.cols[c].values->ptr, (size_t)p.num_rows * w, cudaMemcpyDeviceToDevice, cx.stream));
-        if (any_valid) {
-          if (p.cols[c].validity) B200Q_CUDA(cudaMemcpyAsync((uint8_t*)b->valid_bytes[c]->ptr + at, p.cols[c].validity->ptr, (size_t)p.num_rows, cudaMemcpyDeviceToDevice, cx.stream));
-          else B200Q_CUDA(cudaMemsetAsync((uint8_t*)b->valid_bytes[c]->ptr + at, 1, (size_t)p.num_rows, cx.stream));
-        }
-        at += p.num_rows;
-      }
-    }
-    parts_.clear();
+    b->cols = concat(cx, in_schema, std::move(parts_));
     // table: a power of two >= 2 x rows slots
     uint64_t cap = 1024;
     while (cap < (uint64_t)total * 2) cap <<= 1;
@@ -157,15 +121,14 @@ class JoinBuildStage : public Stage, public JoinBuildResult {
       for (int i = 0; i < k.nkeys; i++) {
         const size_t c = (size_t)keys_[(size_t)i]->col_index;
         k.phys[i] = (uint8_t)phys_of(in_schema.fields[c].type);
-        k.col[i].values = b->values[c]->ptr; k.col[i].validity = nullptr; k.col[i].bit_offset = 0;
+        k.col[i].values = b->cols.values[c]->ptr; k.col[i].validity = nullptr; k.col[i].bit_offset = 0;
       }
       // NULL keys: the build kernel reads validity bitmaps; the side keeps bytes -> pack the keys' bytes once
       std::vector<DevMemP> key_bits;
       for (int i = 0; i < k.nkeys; i++) {
         const size_t c = (size_t)keys_[(size_t)i]->col_index;
-        if (!b->valid_bytes[c]) continue;
-        DevMemP bits = DevMem::alloc(bitmap_bytes(total), cx.stream, true);
-        cx.m.launches += launch_pack_valid((const uint8_t*)b->valid_bytes[c]->ptr, (uint32_t*)bits->ptr, total, cx.stream);
+        if (!b->cols.valid[c]) continue;
+        DevMemP bits = pack_bits(cx, b->cols.valid[c]->ptr, total);
         k.col[i].validity = (const uint8_t*)bits->ptr; key_bits.push_back(bits);
       }
       B200Q_CUDA(cudaEventRecord(cx.ev0, cx.stream));
@@ -173,7 +136,8 @@ class JoinBuildStage : public Stage, public JoinBuildResult {
       B200Q_CUDA(cudaEventRecord(cx.ev1, cx.stream));
       B200Q_CUDA(cudaMemcpyAsync(&b->max_dup, b->t_stats->ptr, 4, cudaMemcpyDeviceToHost, cx.stream));
       B200Q_CUDA(cudaStreamSynchronize(cx.stream));
-      float ms = 0; B200Q_CUDA(cudaEventElapsedTime(&ms, cx.ev0, cx.ev1)); cx.m.gpu_ms += ms; cx.m.hot_ms += ms; cx.m.hot_rows += total; cx.m.hot_launches++; cx.m.fast_launches++;
+      add_kernel_time(cx, total, true);
+      cx.m.fast_launches++;
     }
     if (total == 0) { JoinKeys k0{}; cx.m.launches += launch_join_build(k0, 0, t, cx.stream); }      // an empty map side still needs its (all-empty) probe view
     B200Q_CUDA(cudaStreamSynchronize(cx.stream));           // probe ops run on their own streams
@@ -241,29 +205,20 @@ class JoinProbeStage : public Stage, public JoinProbeAttach {
   void need_built(OpContext& cx) {
     if (!built_) throw ExecError(B200Q_ERR_STATE, "join: no build side attached (b200q_op_attach_build) before the first probe batch");
     if (built_->device != cx.device) throw ExecError(B200Q_ERR_INVALID_ARG, "join: the build side lives on another device");
-    if (!map_joined_ && (build_outer_ || (semi_like_ && !probe_is_join_side_))) map_joined_ = DevMem::alloc((size_t)built_->rows + 16, cx.stream, true);
+    if (!map_joined_ && (build_outer_ || (semi_like_ && !probe_is_join_side_))) map_joined_ = DevMem::alloc((size_t)built_->cols.rows + 16, cx.stream, true);
   }
 
-  using Src = GatherSrc;
-  std::vector<DevColumn> gather_all(OpContext& cx, const std::vector<Src>& srcs, const uint32_t* idx, int64_t n) { return gather_columns(cx, srcs, idx, n); }
   std::vector<DevColumn> gather_probe(OpContext& cx, const DevBatch& in, const uint32_t* idx, int64_t n, bool nil_possible) {
-    std::vector<Src> srcs;
-    for (auto& s : in.cols) {
-      const int w = s.type.byte_width();
-      srcs.push_back(Src{s.type, (const uint8_t*)s.values->ptr + (size_t)s.offset * w, s.validity ? (const uint8_t*)s.validity->ptr : nullptr, (uint32_t)s.offset, nullptr, nil_possible || (bool)s.validity});
-    }
-    return gather_all(cx, srcs, idx, n);
+    std::vector<GatherSrc> srcs;
+    for (auto& c : in.cols) srcs.push_back(gather_src_of(c, nil_possible));
+    return gather_columns(cx, srcs, idx, n);
   }
   std::vector<DevColumn> gather_build(OpContext& cx, const uint32_t* idx, int64_t n, bool nil_possible) {
-    std::vector<Src> srcs;
+    const ByteCols& b = built_->cols;
+    std::vector<GatherSrc> srcs;
     for (size_t c = 0; c < built_->schema.fields.size(); c++)
-      srcs.push_back(Src{built_->schema.fields[c].type, built_->values[c]->ptr, nullptr, 0, built_->valid_bytes[c] ? (const uint8_t*)built_->valid_bytes[c]->ptr : nullptr, nil_possible || (bool)built_->valid_bytes[c]});
-    return gather_all(cx, srcs, idx, n);
-  }
-  std::vector<DevColumn> null_columns(OpContext& cx, const SchemaDef& s, int64_t n) {
-    std::vector<DevColumn> out;
-    for (auto& f : s.fields) { DevColumn o; o.type = f.type; o.values = DevMem::alloc((size_t)n * f.type.byte_width() + 16, cx.stream, true); o.validity = DevMem::alloc(bitmap_bytes(n), cx.stream, true); out.push_back(o); }
-    return out;
+      srcs.push_back(GatherSrc{built_->schema.fields[c].type, b.values[c]->ptr, nullptr, 0, b.valid[c] ? (const uint8_t*)b.valid[c]->ptr : nullptr, nil_possible || (bool)b.valid[c]});
+    return gather_columns(cx, srcs, idx, n);
   }
   void emit(std::vector<DevBatch>& outs, std::vector<DevColumn> pcols, std::vector<DevColumn> bcols, int64_t n) {
     DevBatch ob; ob.num_rows = n;
@@ -286,12 +241,7 @@ class JoinProbeStage : public Stage, public JoinProbeAttach {
 
   void push(OpContext& cx, DevBatch& in, std::vector<DevBatch>& outs) override {
     need_built(cx);
-    const int64_t step = 1LL << 26;                    // bounds the per-launch index vectors / output columns
-    for (int64_t r0 = 0; r0 < in.num_rows; r0 += step) {
-      DevBatch part; part.num_rows = std::min(step, in.num_rows - r0);
-      for (auto& c : in.cols) { DevColumn p = c; p.offset = c.offset + r0; part.cols.push_back(p); }
-      probe(cx, part, outs);
-    }
+    for_each_window(in, 1LL << 26, [&](DevBatch& part) { probe(cx, part, outs); });      // bounds the per-launch index vectors / output columns
   }
 
   void probe(OpContext& cx, DevBatch& in, std::vector<DevBatch>& outs) {
@@ -333,13 +283,14 @@ class JoinProbeStage : public Stage, public JoinProbeAttach {
         bc.ncols = (int)built_->schema.fields.size();
         for (int c = 0; c < bc.ncols; c++) {
           GatherCol& g = bc.col[c];
-          g.src = built_->values[(size_t)c]->ptr; g.vbits = nullptr; g.bit_offset = 0; g.vbytes = built_->valid_bytes[(size_t)c] ? (const uint8_t*)built_->valid_bytes[(size_t)c]->ptr : nullptr;
-          out_col(built_->schema.fields[(size_t)c].type, probe_outer_ || built_->valid_bytes[(size_t)c], g, bcols, bvb);
+          const DevMemP& vb = built_->cols.valid[(size_t)c];
+          g.src = built_->cols.values[(size_t)c]->ptr; g.vbits = nullptr; g.bit_offset = 0; g.vbytes = vb ? (const uint8_t*)vb->ptr : nullptr;
+          out_col(built_->schema.fields[(size_t)c].type, probe_outer_ || vb, g, bcols, bvb);
         }
         cx.m.launches += launch_join_probe_fused((const uint32_t*)head->ptr, n, probe_outer_ ? 1 : 0, (unsigned long long*)cursor->ptr, pc, bc, mark, cx.stream);
         auto pack = [&](std::vector<DevColumn>& cols, std::vector<DevMemP>& vbs) {
           for (size_t c = 0; c < cols.size(); c++)
-            if (vbs[c]) { cols[c].validity = DevMem::alloc(bitmap_bytes(total), cx.stream, true); cx.m.launches += launch_pack_valid((const uint8_t*)vbs[c]->ptr, (uint32_t*)cols[c].validity->ptr, total, cx.stream); }
+            if (vbs[c]) cols[c].validity = pack_bits(cx, vbs[c]->ptr, total);
         };
         pack(pcols, pvb); pack(bcols, bvb);
         emit(outs, pcols, bcols, total);
@@ -359,7 +310,7 @@ class JoinProbeStage : public Stage, public JoinProbeAttach {
             o.values = DevMem::alloc((size_t)n * w + 16, cx.stream); o.offset = 0;
             B200Q_CUDA(cudaMemcpyAsync(o.values->ptr, (const uint8_t*)c.values->ptr + (size_t)c.offset * w, (size_t)n * w, cudaMemcpyDeviceToDevice, cx.stream));
             if (c.validity) { DevMemP vb = DevMem::alloc((size_t)n + 16, cx.stream); cx.m.launches += launch_unpack_bits((const uint8_t*)c.validity->ptr, (uint32_t)c.offset, n, (uint8_t*)vb->ptr, cx.stream);
-                              o.validity = DevMem::alloc(bitmap_bytes(n), cx.stream, true); cx.m.launches += launch_pack_valid((const uint8_t*)vb->ptr, (uint32_t*)o.validity->ptr, n, cx.stream); }
+                              o.validity = pack_bits(cx, vb->ptr, n); }
           } else {                                     // the caller's buffers are released after push: copy
             const int w = c.type.byte_width();
             o.values = DevMem::alloc((size_t)n * w + 16, cx.stream);
@@ -371,8 +322,7 @@ class JoinProbeStage : public Stage, public JoinProbeAttach {
         DevMemP head = DevMem::alloc((size_t)n * 4 + 16, cx.stream), fb = DevMem::alloc((size_t)n + 16, cx.stream);
         cx.m.launches += launch_join_probe_count(k, n, built_->table, 0, (uint32_t*)head->ptr, nullptr, cx.stream);
         cx.m.launches += launch_join_match_bytes((const uint32_t*)head->ptr, n, (uint8_t*)fb->ptr, cx.stream);
-        DevColumn ex; ex.type.id = T_BOOL; ex.values = DevMem::alloc(bitmap_bytes(n), cx.stream, true);
-        cx.m.launches += launch_pack_valid((const uint8_t*)fb->ptr, (uint32_t*)ex.values->ptr, n, cx.stream);
+        DevColumn ex; ex.type.id = T_BOOL; ex.values = pack_bits(cx, fb->ptr, n);
         ob.cols.push_back(ex);
         outs.push_back(std::move(ob));
       } else {                                         // LeftSemi / LeftAnti with the probe side as the join side (semi_join.rs:243-251)
@@ -384,13 +334,14 @@ class JoinProbeStage : public Stage, public JoinProbeAttach {
     }
     B200Q_CUDA(cudaEventRecord(cx.ev1, cx.stream));
     B200Q_CUDA(cudaStreamSynchronize(cx.stream));
-    { float ms = 0; B200Q_CUDA(cudaEventElapsedTime(&ms, cx.ev0, cx.ev1)); cx.m.gpu_ms += ms; cx.m.hot_ms += ms; cx.m.hot_rows += n; cx.m.hot_launches++; cx.m.fast_launches++; }
+    add_kernel_time(cx, n, true);
+    cx.m.fast_launches++;
   }
 
   void finish(OpContext& cx, std::vector<DevBatch>& outs) override {
     if (!built_) { if (cx.m.input_rows == 0) return; throw ExecError(B200Q_ERR_STATE, "join: no build side attached"); }
     need_built(cx);
-    const int64_t nb = built_->rows;
+    const int64_t nb = built_->cols.rows;
     if (nb == 0 || !map_joined_) return;
     if (!semi_like_ && build_outer_) {                 // unjoined build rows next to NULL probe columns (full_join.rs:322-362)
       DevMemP fl = DevMem::alloc((size_t)nb * 4 + 16, cx.stream), offs;
@@ -413,8 +364,7 @@ class JoinProbeStage : public Stage, public JoinProbeAttach {
         scan(cx, (const int32_t*)all->ptr, nb, offs);
         cx.m.launches += launch_join_compact_indices((const int32_t*)all->ptr, (const int32_t*)offs->ptr, nb, (uint32_t*)idn->ptr, cx.stream);   // identity indices
         DevBatch ob; ob.num_rows = nb; ob.cols = gather_build(cx, (const uint32_t*)idn->ptr, nb, false);
-        DevColumn ex; ex.type.id = T_BOOL; ex.values = DevMem::alloc(bitmap_bytes(nb), cx.stream, true);
-        cx.m.launches += launch_pack_valid((const uint8_t*)map_joined_->ptr, (uint32_t*)ex.values->ptr, nb, cx.stream);
+        DevColumn ex; ex.type.id = T_BOOL; ex.values = pack_bits(cx, map_joined_->ptr, nb);
         ob.cols.push_back(ex);
         outs.push_back(std::move(ob));
       } else {

@@ -35,8 +35,6 @@ void set_file_reader(b200q_file_reader_fn fn, void* ctx) { g_reader = fn; g_read
 
 namespace {
 
-inline size_t bitmap_bytes(int64_t n) { return (size_t)((n + 31) / 32) * 4; }
-
 struct FileIo {                                   // positional reads: the column chunks of a row group are read by concurrent host threads
   std::string path; int fd = -1; int64_t size = -1; std::mutex mu;
   explicit FileIo(const std::string& p, uint64_t declared_size) : path(p) {
@@ -202,12 +200,11 @@ DevColumn decode_chunk(OpContext& cx, const PreparedChunk& pc, const PqColumnSch
     d_ord = DevMem::alloc((size_t)(rows + 1) * 4, cx.stream);
     cx.m.launches += launch_bytes_to_flags((const uint8_t*)d_valid->ptr, rows, 0, (int32_t*)fl->ptr, cx.stream);
     cx.m.launches += launch_exclusive_scan_i32((const int32_t*)fl->ptr, (int32_t*)d_ord->ptr, rows, (int32_t*)sums->ptr, cx.stream);
-    col.validity = DevMem::alloc(bitmap_bytes(rows), cx.stream, true);
-    cx.m.launches += launch_pack_valid((const uint8_t*)d_valid->ptr, (uint32_t*)col.validity->ptr, rows, cx.stream);
+    col.validity = pack_bits(cx, d_valid->ptr, rows);
   }
   DevMemP out = DevMem::alloc((size_t)rows * out_w + 16, cx.stream);
   cx.m.launches += launch_pq_decode(sp, any_null ? (const uint8_t*)d_valid->ptr : nullptr, any_null ? (const int32_t*)d_ord->ptr : nullptr, rows, out->ptr, (int*)d_err->ptr, cx.stream);
-  if (cs.type == PQ_BOOLEAN) { col.values = DevMem::alloc(bitmap_bytes(rows), cx.stream, true); cx.m.launches += launch_pack_valid((const uint8_t*)out->ptr, (uint32_t*)col.values->ptr, rows, cx.stream); }
+  if (cs.type == PQ_BOOLEAN) col.values = pack_bits(cx, out->ptr, rows);
   else col.values = out;
   if (dbg) { cudaStreamSynchronize(cx.stream); g_dbg_kernel_ms += hnow() - td1; }
   return col;

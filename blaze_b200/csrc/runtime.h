@@ -7,6 +7,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <deque>
 #include <functional>
 #include <memory>
@@ -167,6 +168,40 @@ struct SmjRightAttach {
 
 // a column as the kernels see it (stages.cu)
 DevCol dev_col_of(const DevColumn& c);
+
+// ---- batch plumbing shared by the stages (stages.cu) ----------------------------------------------------------------------
+// a validity / Boolean bitmap of n rows: whole 32-bit words, as pack_valid_kernel writes them
+inline size_t bitmap_bytes(int64_t n) { return (size_t)((n + 31) / 32) * 4; }
+// n bytes (one per row, nonzero = set) packed into a new bitmap; every word is written, so the allocation is not zeroed
+DevMemP pack_bits(OpContext& cx, const void* bytes, int64_t n);
+// contiguous columns with validity as one byte per row: values rows*w + 16 bytes, valid rows + 16 (the 16-byte tail serves the
+// kernels' 128-bit loads); valid[c] is null when no row of column c can be NULL
+struct ByteCols { int64_t rows = 0; std::vector<DevMemP> values, valid; };
+// Arrow-form batches (any offset, bit validity), or ByteCols, copied one after another into one ByteCols; the rows of a part
+// without validity read as valid.  concat releases its parts.
+ByteCols to_byte_cols(OpContext& cx, const SchemaDef& schema, const std::vector<const DevBatch*>& parts);
+ByteCols concat(OpContext& cx, const SchemaDef& schema, std::vector<ByteCols>&& parts);
+// n rows of NULL in every column of `schema` (zeroed values and bitmaps)
+std::vector<DevColumn> null_columns(OpContext& cx, const SchemaDef& schema, int64_t n);
+// after the stream sync: cx.ev0 -> cx.ev1 into gpu_ms, and when `hot` also into the hot_kernel_* metrics over `rows` rows
+void add_kernel_time(OpContext& cx, int64_t rows, bool hot);
+// whether a column may be passed on without a copy: offset 0 and every buffer owned by the op or kept alive by an owner
+// (borrowed caller memory, push_device, is only valid until the batch is released)
+inline bool kept_alive(const DevMemP& m) { return !m || m->owned || m->owner; }
+inline bool forwardable(const DevColumn& c) { return c.offset == 0 && kept_alive(c.values) && kept_alive(c.validity) && kept_alive(c.offsets); }
+// f(window) for consecutive windows of at most `rows` rows of `in` (the same buffers at moved offsets)
+template <class F> void for_each_window(const DevBatch& in, int64_t rows, F&& f) {
+  for (int64_t r0 = 0; r0 < in.num_rows; r0 += rows) {
+    DevBatch part; part.num_rows = std::min(rows, in.num_rows - r0);
+    for (auto& c : in.cols) { DevColumn p = c; p.offset = c.offset + r0; part.cols.push_back(p); }
+    f(part);
+  }
+}
+// an Arrow-form column (bit validity at its offset) as a gather source
+inline GatherSrc gather_src_of(const DevColumn& c, bool nil_possible) {
+  return GatherSrc{c.type, (const uint8_t*)c.values->ptr + (size_t)c.offset * c.type.byte_width(), c.validity ? (const uint8_t*)c.validity->ptr : nullptr,
+                   (uint32_t)c.offset, nullptr, nil_possible || (bool)c.validity};
+}
 
 // helpers of the C ABI layer (capi.cu) shared with exchange.cu
 DType type_of_format(const char* arrow_format);

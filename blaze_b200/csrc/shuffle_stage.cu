@@ -129,7 +129,7 @@ class ShuffleWriteStage : public Stage, public ShuffleResult {
     B200Q_CUDA(cudaMemcpyAsync(ch.part_rows.data(), d_counts, (size_t)P_ * 8, cudaMemcpyDeviceToHost, cx.stream));
     B200Q_CUDA(cudaMemcpyAsync(ch.part_off.data(), d_part_off, (size_t)(P_ + 1) * 8, cudaMemcpyDeviceToHost, cx.stream));
     B200Q_CUDA(cudaStreamSynchronize(cx.stream));
-    { float ms = 0; B200Q_CUDA(cudaEventElapsedTime(&ms, cx.ev0, cx.ev1)); cx.m.gpu_ms += ms; if (cx.cur_stage == 0) { cx.m.hot_ms += ms; cx.m.hot_rows += n; cx.m.hot_launches++; } }
+    add_kernel_time(cx, n, cx.cur_stage == 0);
     const unsigned long long total = ch.part_off[(size_t)P_];
     if (total > cap) throw ExecError(B200Q_ERR_EXECUTION, "internal: encoded shuffle chunk larger than its bound");
     if (cx.conf.shuffle_output_on_device) ch.dev = d_out;
@@ -238,7 +238,7 @@ class ShuffleWriteStage : public Stage, public ShuffleResult {
     B200Q_CUDA(cudaMemcpyAsync(ch.rec_off.data(), vl.rec_off, (size_t)(R + 1) * 8, cudaMemcpyDeviceToHost, cx.stream));
     B200Q_CUDA(cudaMemcpyAsync(&err, vl.err, 4, cudaMemcpyDeviceToHost, cx.stream));
     B200Q_CUDA(cudaStreamSynchronize(cx.stream));
-    { float ms = 0; B200Q_CUDA(cudaEventElapsedTime(&ms, cx.ev0, cx.ev1)); cx.m.gpu_ms += ms; if (cx.cur_stage == 0) { cx.m.hot_ms += ms; cx.m.hot_rows += n; cx.m.hot_launches++; } }
+    add_kernel_time(cx, n, cx.cur_stage == 0);
     if (err & 1) throw ExecError(B200Q_ERR_UNSUPPORTED, "one shuffle record would carry more than INT32_MAX (2^31 - 1) bytes of Binary data, "
                                                         "the limit of the reader's 32-bit offsets; push smaller batches or lower batch_size");
     const unsigned long long total = ch.part_off[(size_t)P_];

@@ -19,8 +19,6 @@ namespace b200q {
 
 namespace {
 
-inline size_t bitmap_bytes(int64_t n) { return (size_t)((n + 31) / 32) * 4; }
-
 enum { SJ_INNER = 0, SJ_LEFT, SJ_RIGHT, SJ_FULL, SJ_SEMI, SJ_ANTI, SJ_EXISTENCE };   // protobuf JoinType (auron.proto:475-483)
 
 SortKeyCol key_col(const DType& t, const void* values, const uint8_t* vbits, uint32_t bit_offset, const uint8_t* vbytes, const PlanNode::SortOptionsDef& o) {
@@ -98,30 +96,18 @@ class SmjStage : public Stage, public SmjRightAttach {
     const size_t ncols = right_.fields.size();
     std::vector<GatherSrc> src(ncols);
     std::vector<DevMemP> keep;
-    for (size_t c = 0; c < ncols; c++) {
-      const DType& t = right_.fields[c].type;
-      const size_t w = (size_t)t.byte_width();
-      GatherSrc& g = src[c]; g = GatherSrc{t, nullptr, nullptr, 0, nullptr, false};
-      if (parts.size() == 1) {                      // one batch (what a SortExec emits): used where it lies
+    for (size_t c = 0; c < ncols; c++) src[c] = GatherSrc{right_.fields[c].type, nullptr, nullptr, 0, nullptr, false};
+    if (parts.size() == 1) {                        // one batch (what a SortExec emits): used where it lies
+      for (size_t c = 0; c < ncols; c++) {
         const DevColumn& dc = parts[0]->cols[c];
-        g.values = (const uint8_t*)dc.values->ptr + (size_t)dc.offset * w; keep.push_back(dc.values);
-        if (dc.validity) { g.vbits = (const uint8_t*)dc.validity->ptr; g.bit_offset = (uint32_t)dc.offset; g.may_be_null = true; keep.push_back(dc.validity); }
-      } else if (parts.size() > 1) {                // several: concatenated once, validity as one byte per row
-        DevMemP v = DevMem::alloc((size_t)m * w + 16, cx.stream), vb;
-        bool any = false; for (auto* p : parts) any = any || p->cols[c].validity;
-        if (any) vb = DevMem::alloc((size_t)m + 16, cx.stream);
-        int64_t at = 0;
-        for (auto* p : parts) {
-          const DevColumn& dc = p->cols[c];
-          B200Q_CUDA(cudaMemcpyAsync((uint8_t*)v->ptr + (size_t)at * w, (const uint8_t*)dc.values->ptr + (size_t)dc.offset * w, (size_t)p->num_rows * w, cudaMemcpyDeviceToDevice, cx.stream));
-          if (any) {
-            if (dc.validity) cx.m.launches += launch_unpack_bits((const uint8_t*)dc.validity->ptr, (uint32_t)dc.offset, p->num_rows, (uint8_t*)vb->ptr + at, cx.stream);
-            else B200Q_CUDA(cudaMemsetAsync((uint8_t*)vb->ptr + at, 1, (size_t)p->num_rows, cx.stream));
-          }
-          at += p->num_rows;
-        }
-        g.values = v->ptr; keep.push_back(v);
-        if (any) { g.vbytes = (const uint8_t*)vb->ptr; g.may_be_null = true; keep.push_back(vb); }
+        src[c] = gather_src_of(dc, false); keep.push_back(dc.values);
+        if (dc.validity) keep.push_back(dc.validity);
+      }
+    } else if (parts.size() > 1) {                  // several: concatenated once, validity as one byte per row
+      const ByteCols bc = to_byte_cols(cx, right_, parts);
+      for (size_t c = 0; c < ncols; c++) {
+        src[c].values = bc.values[c]->ptr; keep.push_back(bc.values[c]);
+        if (bc.valid[c]) { src[c].vbytes = (const uint8_t*)bc.valid[c]->ptr; src[c].may_be_null = true; keep.push_back(bc.valid[c]); }
       }
     }
     // normalise the right keys once and check their order
@@ -140,12 +126,7 @@ class SmjStage : public Stage, public SmjRightAttach {
 
   void push(OpContext& cx, DevBatch& in, std::vector<DevBatch>& outs) override {
     if (!attached_) throw ExecError(B200Q_ERR_STATE, "SortMergeJoinExec: no right side attached (b200q_op_attach_right) before the first left batch");
-    const int64_t step = 1LL << 26;                  // bounds the per-launch index vectors
-    for (int64_t r0 = 0; r0 < in.num_rows; r0 += step) {
-      DevBatch part; part.num_rows = std::min(step, in.num_rows - r0);
-      for (auto& c : in.cols) { DevColumn p = c; p.offset = c.offset + r0; part.cols.push_back(p); }
-      join_batch(cx, part, outs);
-    }
+    for_each_window(in, 1LL << 26, [&](DevBatch& part) { join_batch(cx, part, outs); });      // bounds the per-launch index vectors
   }
 
   void join_batch(OpContext& cx, DevBatch& in, std::vector<DevBatch>& outs) {
@@ -191,7 +172,8 @@ class SmjStage : public Stage, public SmjRightAttach {
       e.nw = nw; e.U = (const unsigned long long*)U->ptr; e.matched = (const uint8_t*)matched_->ptr;
       settled_ = s_new;
     }
-    { float ms = 0; B200Q_CUDA(cudaEventElapsedTime(&ms, cx.ev0, cx.ev1)); cx.m.gpu_ms += ms; if (cx.cur_stage == 0) { cx.m.hot_ms += ms; cx.m.hot_rows += n; cx.m.hot_launches++; } cx.m.fast_launches++; }
+    add_kernel_time(cx, n, cx.cur_stage == 0);
+    cx.m.fast_launches++;
     emit_chunks(cx, outs, &in, e, total);
   }
 
@@ -214,21 +196,13 @@ class SmjStage : public Stage, public SmjRightAttach {
       DevBatch ob; ob.num_rows = cnt;
       if (in) {
         std::vector<GatherSrc> ls;
-        for (auto& c : in->cols) {
-          const int w = c.type.byte_width();
-          ls.push_back(GatherSrc{c.type, (const uint8_t*)c.values->ptr + (size_t)c.offset * w, c.validity ? (const uint8_t*)c.validity->ptr : nullptr, (uint32_t)c.offset, nullptr, right_outer_ || (bool)c.validity});
-        }
+        for (auto& c : in->cols) ls.push_back(gather_src_of(c, right_outer_));
         ob.cols = gather_columns(cx, ls, (const uint32_t*)pidx->ptr, cnt);
       } else {                                       // right-only rows: NULL left columns
-        for (auto& f : left_.fields) {
-          DevColumn o; o.type = f.type;
-          o.values = DevMem::alloc((size_t)cnt * f.type.byte_width() + 16, cx.stream, true); o.validity = DevMem::alloc(bitmap_bytes(cnt), cx.stream, true);
-          ob.cols.push_back(o);
-        }
+        ob.cols = null_columns(cx, left_, cnt);
       }
       if (jt_ == SJ_EXISTENCE) {
-        DevColumn x; x.type.id = T_BOOL; x.values = DevMem::alloc(bitmap_bytes(cnt), cx.stream, true);
-        cx.m.launches += launch_pack_valid((const uint8_t*)ex->ptr, (uint32_t*)x.values->ptr, cnt, cx.stream);
+        DevColumn x; x.type.id = T_BOOL; x.values = pack_bits(cx, ex->ptr, cnt);
         ob.cols.push_back(x);
       } else if (!semi_like_) {
         std::vector<GatherSrc> rs = rsrc_;

@@ -17,13 +17,11 @@ namespace b200q {
 
 namespace {
 
-inline size_t bitmap_bytes(int64_t n) { return (size_t)((n + 31) / 32) * 4; }
-
 class SortStage : public Stage {
   struct Key { int col; bool desc, nulls_first; };
   std::vector<Key> keys_;
   int64_t fetch_ = -1;
-  std::vector<DevBatch> parts_;
+  std::vector<ByteCols> parts_;                                       // owned copies of the pushed batches
 
  public:
   SortStage(OpContext&, const SchemaDef& in, const PlanNode& node) {
@@ -40,41 +38,18 @@ class SortStage : public Stage {
   }
 
   void push(OpContext& cx, DevBatch& in, std::vector<DevBatch>&) override {
-    const int64_t n = in.num_rows;
-    if (n == 0) return;                                                 // sort_exec.rs:627-629
-    DevBatch own; own.num_rows = n;
-    for (auto& c : in.cols) {
-      DevColumn o; o.type = c.type;
-      const size_t w = (size_t)c.type.byte_width();
-      o.values = DevMem::alloc((size_t)n * w, cx.stream);
-      B200Q_CUDA(cudaMemcpyAsync(o.values->ptr, (const uint8_t*)c.values->ptr + (size_t)c.offset * w, (size_t)n * w, cudaMemcpyDeviceToDevice, cx.stream));
-      if (c.validity) { o.validity = DevMem::alloc((size_t)n, cx.stream); cx.m.launches += launch_unpack_bits((const uint8_t*)c.validity->ptr, (uint32_t)c.offset, n, (uint8_t*)o.validity->ptr, cx.stream); }
-      own.cols.push_back(o);
-    }
-    parts_.push_back(std::move(own));
+    if (in.num_rows == 0) return;                                       // sort_exec.rs:627-629
+    parts_.push_back(to_byte_cols(cx, in_schema, {&in}));              // the caller's buffers are released when push returns
   }
 
   void finish(OpContext& cx, std::vector<DevBatch>& outs) override {
     int64_t n = 0;
-    for (auto& p : parts_) n += p.num_rows;
+    for (auto& p : parts_) n += p.rows;
     if (n == 0) return;
     if (n > 0x7FFFFFFFLL) throw ExecError(B200Q_ERR_UNSUPPORTED, "SortExec: more than 2^31-1 rows");
     const size_t ncols = in_schema.fields.size();
-    std::vector<DevMemP> values(ncols), valid(ncols);
-    for (size_t c = 0; c < ncols; c++) {
-      const size_t w = (size_t)in_schema.fields[c].type.byte_width();
-      values[c] = DevMem::alloc((size_t)n * w + 16, cx.stream);
-      bool any = false; for (auto& p : parts_) any = any || p.cols[c].validity;
-      if (any) valid[c] = DevMem::alloc((size_t)n + 16, cx.stream);
-      int64_t at = 0;
-      for (auto& p : parts_) {
-        B200Q_CUDA(cudaMemcpyAsync((uint8_t*)values[c]->ptr + (size_t)at * w, p.cols[c].values->ptr, (size_t)p.num_rows * w, cudaMemcpyDeviceToDevice, cx.stream));
-        if (any) { if (p.cols[c].validity) B200Q_CUDA(cudaMemcpyAsync((uint8_t*)valid[c]->ptr + at, p.cols[c].validity->ptr, (size_t)p.num_rows, cudaMemcpyDeviceToDevice, cx.stream));
-                   else B200Q_CUDA(cudaMemsetAsync((uint8_t*)valid[c]->ptr + at, 1, (size_t)p.num_rows, cx.stream)); }
-        at += p.num_rows;
-      }
-    }
-    parts_.clear();
+    const ByteCols cols = concat(cx, in_schema, std::move(parts_));
+    const std::vector<DevMemP> &values = cols.values, &valid = cols.valid;
     // ---- sort a permutation ------------------------------------------------------------------------------------------
     const int64_t ntiles = sort_num_tiles(n);
     DevMemP keyA = DevMem::alloc((size_t)n * 8, cx.stream), keyB = DevMem::alloc((size_t)n * 8, cx.stream);
@@ -124,13 +99,14 @@ class SortStage : public Stage {
         DevMemP ob_valid = valid[c] ? DevMem::alloc((size_t)m + 16, cx.stream) : nullptr;
         cx.m.launches += launch_join_gather(values[c]->ptr, nullptr, 0, valid[c] ? (const uint8_t*)valid[c]->ptr : nullptr, w, (const uint32_t*)idxA->ptr, m, o.values->ptr,
                                             ob_valid ? (uint8_t*)ob_valid->ptr : nullptr, cx.stream);
-        if (ob_valid) { o.validity = DevMem::alloc(bitmap_bytes(m), cx.stream, true); cx.m.launches += launch_pack_valid((const uint8_t*)ob_valid->ptr, (uint32_t*)o.validity->ptr, m, cx.stream); }
+        if (ob_valid) o.validity = pack_bits(cx, ob_valid->ptr, m);
         ob.cols.push_back(o);
       }
       outs.push_back(std::move(ob));
     }
     B200Q_CUDA(cudaStreamSynchronize(cx.stream));
-    { float ms = 0; B200Q_CUDA(cudaEventElapsedTime(&ms, cx.ev0, cx.ev1)); cx.m.gpu_ms += ms; if (cx.cur_stage == 0) { cx.m.hot_ms += ms; cx.m.hot_rows += n; cx.m.hot_launches++; } cx.m.fast_launches++; }
+    add_kernel_time(cx, n, cx.cur_stage == 0);
+    cx.m.fast_launches++;
   }
 };
 

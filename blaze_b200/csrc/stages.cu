@@ -8,6 +8,7 @@
 
 #include "runtime.h"
 #include "kernels_fast.cuh"
+#include "kernels_join.cuh"
 
 namespace b200q {
 
@@ -60,8 +61,6 @@ DevMemP DevMem::borrow(const void* p, size_t bytes, std::shared_ptr<void> owner)
   return m;
 }
 
-static inline size_t bitmap_bytes(int64_t n) { return (size_t)((n + 31) / 32) * 4; }
-
 DevCol dev_col_of(const DevColumn& c) {
   DevCol d{};
   const int w = c.type.byte_width();
@@ -71,6 +70,70 @@ DevCol dev_col_of(const DevColumn& c) {
   d.bit_offset = (uint32_t)c.offset;
   if (c.offset > 0xFFFFFFFFLL) throw ExecError(B200Q_ERR_UNSUPPORTED, "column offset beyond 2^32 rows");
   return d;
+}
+
+DevMemP pack_bits(OpContext& cx, const void* bytes, int64_t n) {
+  DevMemP bits = DevMem::alloc(bitmap_bytes(n), cx.stream);
+  cx.m.launches += launch_pack_valid((const uint8_t*)bytes, (uint32_t*)bits->ptr, n, cx.stream);
+  return bits;
+}
+
+ByteCols to_byte_cols(OpContext& cx, const SchemaDef& schema, const std::vector<const DevBatch*>& parts) {
+  ByteCols out;
+  for (auto* p : parts) out.rows += p->num_rows;
+  for (size_t c = 0; c < schema.fields.size(); c++) {
+    const size_t w = (size_t)schema.fields[c].type.byte_width();
+    DevMemP v = DevMem::alloc((size_t)out.rows * w + 16, cx.stream), vb;
+    bool any = false; for (auto* p : parts) any = any || p->cols[c].validity;
+    if (any) vb = DevMem::alloc((size_t)out.rows + 16, cx.stream);
+    int64_t at = 0;
+    for (auto* p : parts) {
+      const DevColumn& dc = p->cols[c];
+      B200Q_CUDA(cudaMemcpyAsync((uint8_t*)v->ptr + (size_t)at * w, (const uint8_t*)dc.values->ptr + (size_t)dc.offset * w, (size_t)p->num_rows * w, cudaMemcpyDeviceToDevice, cx.stream));
+      if (dc.validity) cx.m.launches += launch_unpack_bits((const uint8_t*)dc.validity->ptr, (uint32_t)dc.offset, p->num_rows, (uint8_t*)vb->ptr + at, cx.stream);
+      else if (vb) B200Q_CUDA(cudaMemsetAsync((uint8_t*)vb->ptr + at, 1, (size_t)p->num_rows, cx.stream));
+      at += p->num_rows;
+    }
+    out.values.push_back(v); out.valid.push_back(vb);
+  }
+  return out;
+}
+
+ByteCols concat(OpContext& cx, const SchemaDef& schema, std::vector<ByteCols>&& parts) {
+  const std::vector<ByteCols> ps = std::move(parts);           // released (stream-ordered) once copied
+  ByteCols out;
+  for (auto& p : ps) out.rows += p.rows;
+  for (size_t c = 0; c < schema.fields.size(); c++) {
+    const size_t w = (size_t)schema.fields[c].type.byte_width();
+    DevMemP v = DevMem::alloc((size_t)out.rows * w + 16, cx.stream), vb;
+    bool any = false; for (auto& p : ps) any = any || p.valid[c];
+    if (any) vb = DevMem::alloc((size_t)out.rows + 16, cx.stream);
+    int64_t at = 0;
+    for (auto& p : ps) {
+      B200Q_CUDA(cudaMemcpyAsync((uint8_t*)v->ptr + (size_t)at * w, p.values[c]->ptr, (size_t)p.rows * w, cudaMemcpyDeviceToDevice, cx.stream));
+      if (p.valid[c]) B200Q_CUDA(cudaMemcpyAsync((uint8_t*)vb->ptr + at, p.valid[c]->ptr, (size_t)p.rows, cudaMemcpyDeviceToDevice, cx.stream));
+      else if (vb) B200Q_CUDA(cudaMemsetAsync((uint8_t*)vb->ptr + at, 1, (size_t)p.rows, cx.stream));
+      at += p.rows;
+    }
+    out.values.push_back(v); out.valid.push_back(vb);
+  }
+  return out;
+}
+
+std::vector<DevColumn> null_columns(OpContext& cx, const SchemaDef& schema, int64_t n) {
+  std::vector<DevColumn> out;
+  for (auto& f : schema.fields) {
+    DevColumn o; o.type = f.type;
+    o.values = DevMem::alloc((size_t)n * f.type.byte_width() + 16, cx.stream, true); o.validity = DevMem::alloc(bitmap_bytes(n), cx.stream, true);
+    out.push_back(o);
+  }
+  return out;
+}
+
+void add_kernel_time(OpContext& cx, int64_t rows, bool hot) {
+  float ms = 0; B200Q_CUDA(cudaEventElapsedTime(&ms, cx.ev0, cx.ev1));
+  cx.m.gpu_ms += ms;
+  if (hot) { cx.m.hot_ms += ms; cx.m.hot_rows += rows; cx.m.hot_launches++; }
 }
 
 // the program in device memory, its Utf8 constants relocated to their device addresses
@@ -165,12 +228,7 @@ class FilterProjectStage : public Stage {
     const int64_t n = in.num_rows;
     if (n == 0) return;
     if (n > 0x7FFFFFFFLL) throw ExecError(B200Q_ERR_UNSUPPORTED, "batches above 2^31-1 rows must be split by the caller");
-    if (identity_) {
-      bool plain = true;
-      auto ours = [](const DevMemP& m) { return !m || m->owned || m->owner; };          // borrowed caller memory (push_device) is only valid until the batch is released
-      for (auto& c : in.cols) plain = plain && c.offset == 0 && ours(c.values) && ours(c.validity) && ours(c.offsets);
-      if (plain) { outs.push_back(in); return; }
-    }
+    if (identity_ && std::all_of(in.cols.begin(), in.cols.end(), forwardable)) { outs.push_back(in); return; }
     ColTable ct{};
     for (size_t i = 0; i < cp_.used_cols.size(); i++) ct.col[i] = dev_col_of(in.cols[cp_.used_cols[i]]);
     OutTable ot{};
@@ -208,7 +266,7 @@ class FilterProjectStage : public Stage {
     unsigned long long h[4];
     B200Q_CUDA(cudaMemcpyAsync(h, scratch->ptr, 32, cudaMemcpyDeviceToHost, cx.stream));
     B200Q_CUDA(cudaStreamSynchronize(cx.stream));
-    { float ms = 0; B200Q_CUDA(cudaEventElapsedTime(&ms, cx.ev0, cx.ev1)); cx.m.gpu_ms += ms; if (cx.cur_stage == 0) { cx.m.hot_ms += ms; cx.m.hot_rows += n; cx.m.hot_launches++; } }
+    add_kernel_time(cx, n, cx.cur_stage == 0);
     check_device_error_flags((int)h[2]);
     ob.num_rows = (int64_t)h[1];
     if (ob.num_rows == 0) return;                            // sender.send drops empty batches (execution_context.rs:713-716)
@@ -223,14 +281,13 @@ class FilterProjectStage : public Stage {
   // of every column are computed first, so that one host round trip brings back all byte totals before the data is allocated.
   void gather_varlen(OpContext& cx, const DevBatch& in, const uint32_t* sel, DevBatch& res) {
     const int64_t m = res.num_rows;
-    auto ours = [](const DevMemP& p) { return !p || p->owned || p->owner; };           // borrowed caller memory (push_device) must be copied
     struct Job { size_t out; DevCol src; };
     std::vector<Job> jobs;
     for (size_t i = 0; i < out_src_.size(); i++) {
       if (out_src_[i] < 0) continue;
       const DevColumn& c = in.cols[(size_t)out_src_[i]];
       // no filter: share the buffers (imported offsets always start at 0, so the column indexes its own allocation)
-      if (!sel && c.offset == 0 && ours(c.values) && ours(c.offsets) && ours(c.validity)) { res.cols[i] = c; continue; }
+      if (!sel && forwardable(c)) { res.cols[i] = c; continue; }
       jobs.push_back(Job{i, dev_col_of(c)});
     }
     if (jobs.empty()) return;
@@ -1321,16 +1378,16 @@ class AggStage : public Stage {
       DevColumn c; c.type = f.type;
       FrozenField& ff = ft.f[k];
       ff.kind = merge_state_kinds_[k]; ff.width = frozen_width(f.type); ff.phys = phys_of(f.type);
-      if (f.type.id == T_BOOL) { bool_bytes[k] = DevMem::alloc((size_t)n, cx.stream); ff.values = bool_bytes[k]->ptr; c.values = DevMem::alloc(bitmap_bytes(n), cx.stream); }
+      if (f.type.id == T_BOOL) { bool_bytes[k] = DevMem::alloc((size_t)n, cx.stream); ff.values = bool_bytes[k]->ptr; }
       else { c.values = DevMem::alloc((size_t)n * f.type.byte_width(), cx.stream); ff.values = c.values->ptr; }
-      if (f.nullable) { valid_bytes[k] = DevMem::alloc((size_t)n, cx.stream); ff.valid = (const uint8_t*)valid_bytes[k]->ptr; c.validity = DevMem::alloc(bitmap_bytes(n), cx.stream); }
+      if (f.nullable) { valid_bytes[k] = DevMem::alloc((size_t)n, cx.stream); ff.valid = (const uint8_t*)valid_bytes[k]->ptr; }
       state_cols.push_back(c);
     }
     int* d_err = (int*)((unsigned long long*)counters_->ptr + 2);
     cx.m.launches += launch_frozen_read(ft, n, (const int32_t*)bc.offsets->ptr, bc.offset, (const uint8_t*)bc.values->ptr, d_err, cx.stream);
     for (int k = 0; k < ft.nfields; k++) {
-      if (valid_bytes[k]) cx.m.launches += launch_pack_valid((const uint8_t*)valid_bytes[k]->ptr, (uint32_t*)state_cols[k].validity->ptr, n, cx.stream);
-      if (bool_bytes[k]) cx.m.launches += launch_pack_valid((const uint8_t*)bool_bytes[k]->ptr, (uint32_t*)state_cols[k].values->ptr, n, cx.stream);
+      if (valid_bytes[k]) state_cols[k].validity = pack_bits(cx, valid_bytes[k]->ptr, n);
+      if (bool_bytes[k]) state_cols[k].values = pack_bits(cx, bool_bytes[k]->ptr, n);
     }
     B200Q_CUDA(cudaGetLastError());
     // valid_bytes buffers are released stream-ordered after the pack kernels
@@ -1362,9 +1419,9 @@ class AggStage : public Stage {
     for (size_t i = 0; i < emit_.size(); i++) {
       EmitCol ec = emit_[i].ec; const FieldDef& f = emit_[i].field;
       DevColumn c; c.type = f.type;
-      if (f.type.id == T_BOOL) { bool_bytes[i] = DevMem::alloc((size_t)g, cx.stream); ec.values = bool_bytes[i]->ptr; c.values = DevMem::alloc(bitmap_bytes(g), cx.stream); }
+      if (f.type.id == T_BOOL) { bool_bytes[i] = DevMem::alloc((size_t)g, cx.stream); ec.values = bool_bytes[i]->ptr; }
       else { c.values = DevMem::alloc((size_t)g * f.type.byte_width(), cx.stream); ec.values = c.values->ptr; }
-      if (f.nullable) { valid_bytes[i] = DevMem::alloc((size_t)g, cx.stream); ec.valid_bytes = (uint8_t*)valid_bytes[i]->ptr; c.validity = DevMem::alloc(bitmap_bytes(g), cx.stream); }
+      if (f.nullable) { valid_bytes[i] = DevMem::alloc((size_t)g, cx.stream); ec.valid_bytes = (uint8_t*)valid_bytes[i]->ptr; }
       et.col[i] = ec;
       ob.cols.push_back(c);
     }
@@ -1373,8 +1430,8 @@ class AggStage : public Stage {
     if (fs_.dense) cx.m.launches += launch_agg_emit_dense(fs_, et, dmap_, (unsigned long long*)out_count->ptr, cx.stream);
     if (wide) cx.m.launches += launch_tile_wide_emit(ws_, lay_, et, (unsigned long long*)out_count->ptr, cx.stream);
     for (size_t i = 0; i < emit_.size(); i++) {
-      if (valid_bytes[i]) cx.m.launches += launch_pack_valid((const uint8_t*)valid_bytes[i]->ptr, (uint32_t*)ob.cols[i].validity->ptr, g, cx.stream);
-      if (bool_bytes[i]) cx.m.launches += launch_pack_valid((const uint8_t*)bool_bytes[i]->ptr, (uint32_t*)ob.cols[i].values->ptr, g, cx.stream);
+      if (valid_bytes[i]) ob.cols[i].validity = pack_bits(cx, valid_bytes[i]->ptr, g);
+      if (bool_bytes[i]) ob.cols[i].values = pack_bits(cx, bool_bytes[i]->ptr, g);
     }
     B200Q_CUDA(cudaGetLastError());
     if (!final_ && !columnar_) {

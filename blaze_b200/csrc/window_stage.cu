@@ -12,8 +12,6 @@ namespace b200q {
 
 namespace {
 
-inline size_t bitmap_bytes(int64_t n) { return (size_t)((n + 31) / 32) * 4; }
-
 class WindowStage : public Stage {
   WinKeys keys_{};
   std::vector<WinFn> fns_;
@@ -85,10 +83,7 @@ class WindowStage : public Stage {
     for (int k = 0; k < keys.nkeys; k++) keys.k[k].col = dev_col_of(in.cols[(size_t)key_cols_[(size_t)k]]);
     DevBatch ob; ob.num_rows = n;
     // forwarded columns: shared when the op owns them at offset 0 (the identity-path rule), copied otherwise
-    bool plain = true;
-    auto ours = [](const DevMemP& m) { return !m || m->owned || m->owner; };
-    for (size_t i = 0; i < n_fwd_; i++) { const DevColumn& c = in.cols[i]; plain = plain && c.offset == 0 && ours(c.values) && ours(c.validity) && ours(c.offsets); }
-    if (plain) ob.cols.assign(in.cols.begin(), in.cols.begin() + (long)n_fwd_);
+    if (std::all_of(in.cols.begin(), in.cols.begin() + (long)n_fwd_, forwardable)) ob.cols.assign(in.cols.begin(), in.cols.begin() + (long)n_fwd_);
     else {
       // the copy is timed into gpu_ms by the nested stage, but kept out of the hot_kernel_* metrics: those describe this stage's
       // window kernels (and count each input row once)
@@ -127,14 +122,11 @@ class WindowStage : public Stage {
     B200Q_CUDA(cudaGetLastError());
     for (int r = 0; r < 3; r++)
       for (int e : rank_dup_[r]) B200Q_CUDA(cudaMemcpyAsync(wcols[(size_t)e].values->ptr, wcols[(size_t)rank_out_[r]].values->ptr, (size_t)n * 4, cudaMemcpyDeviceToDevice, cx.stream));
-    for (size_t e = 0; e < win_fields_.size(); e++) {
-      if (!valid_bytes[e]) continue;
-      wcols[e].validity = DevMem::alloc(bitmap_bytes(n), cx.stream, true);
-      cx.m.launches += launch_pack_valid((const uint8_t*)valid_bytes[e]->ptr, (uint32_t*)wcols[e].validity->ptr, n, cx.stream);
-    }
+    for (size_t e = 0; e < win_fields_.size(); e++)
+      if (valid_bytes[e]) wcols[e].validity = pack_bits(cx, valid_bytes[e]->ptr, n);
     for (auto& c : wcols) ob.cols.push_back(c);
     B200Q_CUDA(cudaStreamSynchronize(cx.stream));
-    { float ms = 0; B200Q_CUDA(cudaEventElapsedTime(&ms, cx.ev0, cx.ev1)); cx.m.gpu_ms += ms; if (cx.cur_stage == 0) { cx.m.hot_ms += ms; cx.m.hot_rows += n; cx.m.hot_launches++; } }
+    add_kernel_time(cx, n, cx.cur_stage == 0);
     outs.push_back(std::move(ob));
   }
 
