@@ -45,6 +45,42 @@ def assert_same_rows_ordered(gpu_batches, oracle_out, schema):
             assert np.array_equal(gv, ev), f"col {i}: values differ"
 
 
+def parquet_scan(path, table_schema, **kw):
+    """ParquetScanExec over one file; `range=(lo, hi)` scans one byte-range split of it."""
+    return PL.ParquetScanExec(T.from_arrow_schema(table_schema), [(path, 0, kw.pop("range", None))], **kw)
+
+
+def value_slots(a: pa.Array) -> np.ndarray:
+    """the value bits of every slot of a fixed-width array: one bit per row (Boolean), else one row of bytes per row"""
+    buf = np.frombuffer(a.buffers()[1], np.uint8)
+    if a.type == pa.bool_():
+        return np.unpackbits(buf, bitorder="little")[a.offset: a.offset + len(a)]
+    w = a.type.byte_width
+    return buf[a.offset * w: (a.offset + len(a)) * w].reshape(len(a), w)
+
+
+def assert_same_table(got_batches, exp: pa.Table):
+    """The scan's output against libparquet's reading of the same file: same types and validity, and the same bits in every
+    non-NULL slot (float bits too: NaN payloads, -0.0).  libparquet leaves unspecified values under a NULL; the scan writes
+    zero there, and that is checked too."""
+    got = pa.Table.from_batches(got_batches, schema=got_batches[0].schema) if got_batches else exp.slice(0, 0)
+    assert got.num_rows == exp.num_rows, (got.num_rows, exp.num_rows)
+    if not exp.num_rows:
+        return
+    for name in exp.schema.names:
+        g, e = got.column(name).combine_chunks(), exp.column(name).combine_chunks()
+        assert g.type == e.type, (name, g.type, e.type)
+        valid = e.is_valid().to_numpy(zero_copy_only=False)
+        assert np.array_equal(g.is_valid().to_numpy(zero_copy_only=False), valid), f"{name}: validity differs"
+        if g.null_count == len(g) and g.buffers()[1] is None:
+            continue
+        gv, ev = value_slots(g), value_slots(e) if e.null_count < len(e) else None
+        if ev is not None and valid.any():
+            bad = np.flatnonzero(np.any((gv[valid] != ev[valid]).reshape(int(valid.sum()), -1), axis=1))
+            assert not len(bad), f"{name}: {len(bad)} values differ, first at non-NULL ordinal {bad[0]}: {g.filter(e.is_valid())[int(bad[0])]} vs {e.filter(e.is_valid())[int(bad[0])]}"
+        assert not np.any(gv[~valid]), f"{name}: a NULL slot holds a nonzero value"
+
+
 def assert_multiset_equal(gpu_batches, oracle_out, float_cols=(), rtol=1e-6):
     """HashAgg parity = equality of the multiset of rows (assert_batches_sorted_eq!, agg_exec.rs:679);
     columns listed in float_cols are compared within rtol (fp64 SUM/AVG contract), all others bit-exactly."""

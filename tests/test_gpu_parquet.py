@@ -41,26 +41,6 @@ def _table(n, seed, null_frac):
     return pa.Table.from_arrays(list(cols.values()), schema=pa.schema(fields))
 
 
-def _scan(path, table_schema, **kw):
-    schema = T.from_arrow_schema(table_schema)
-    plan = PL.ParquetScanExec(schema, [(path, 0, kw.pop("range", None))], **kw)
-    return plan
-
-
-def _same(got_batches, exp: pa.Table):
-    got = pa.Table.from_batches(got_batches, schema=got_batches[0].schema) if got_batches else exp.slice(0, 0)
-    assert got.num_rows == exp.num_rows
-    for name in exp.schema.names:
-        g, e = got.column(name).combine_chunks(), exp.column(name).combine_chunks()
-        assert g.type == e.type, (name, g.type, e.type)
-        assert g.is_valid().equals(e.is_valid()), f"{name}: validity differs"
-        if pa.types.is_floating(e.type):
-            w = np.int64 if e.type == pa.float64() else np.int32
-            assert np.array_equal(g.fill_null(0).to_numpy(zero_copy_only=False).view(w), e.fill_null(0).to_numpy(zero_copy_only=False).view(w)), name
-        else:
-            assert g.equals(e), f"{name}: values differ"
-
-
 @pytest.mark.parametrize("compression", ["none", "snappy"])
 @pytest.mark.parametrize("dictionary", [True, False])
 @pytest.mark.parametrize("page_version", ["1.0", "2.0"])
@@ -69,9 +49,9 @@ def test_scan_matches_libparquet(tmp_path, compression, dictionary, page_version
     path = str(tmp_path / "t.parquet")
     pq.write_table(t, path, compression=compression, use_dictionary=dictionary, data_page_version=page_version, row_group_size=9_000, data_page_size=16 * 1024,
                    store_decimal_as_integer=True)
-    plan = _scan(path, t.schema)
+    plan = parquet_scan(path, t.schema)
     out = PL.collect(plan)
-    _same(out, pq.read_table(path))
+    assert_same_table(out, pq.read_table(path))
     assert plan.last_metrics["gpu_kernel_launches"] > 0 and plan.last_metrics["input_batches"] == 3          # one device batch per row group
 
 
@@ -85,7 +65,7 @@ def test_required_columns_dictionary_fallback_and_flba_decimals(tmp_path):
     t = t.cast(pa.schema([pa.field(f.name, f.type, False) for f in t.schema]))
     path = str(tmp_path / "t.parquet")
     pq.write_table(t, path, compression="snappy", use_dictionary=True, dictionary_pagesize_limit=64 * 1024, row_group_size=50_000)
-    _same(PL.collect(_scan(path, t.schema)), pq.read_table(path))
+    assert_same_table(PL.collect(parquet_scan(path, t.schema)), pq.read_table(path))
 
 
 def test_projection_pruning_limit_and_filter_above(tmp_path):
@@ -95,25 +75,25 @@ def test_projection_pruning_limit_and_filter_above(tmp_path):
     names = t.schema.names
     proj = [names.index("f64"), names.index("k"), names.index("i32")]
     # projection (subset + reorder)
-    _same(PL.collect(_scan(path, t.schema, projection=proj)), pq.read_table(path, columns=["f64", "k", "i32"]))
+    assert_same_table(PL.collect(parquet_scan(path, t.schema, projection=proj)), pq.read_table(path, columns=["f64", "k", "i32"]))
     # row-group pruning: k is sorted, 8 row groups; `k >= v` must skip the row groups below v, the FilterExec above removes the rest
     v = int(t.column("k")[22_000].as_py())
     pred = E.BinaryExpr(E.Column("k"), "GtEq", E.Literal(v, T.int64))
-    scan = _scan(path, t.schema, projection=proj, pruning_predicates=[pred])
+    scan = parquet_scan(path, t.schema, projection=proj, pruning_predicates=[pred])
     plan = PL.FilterExec([pred], scan)
     out = PL.collect(plan)
     exp = pq.read_table(path, columns=["f64", "k", "i32"]).filter(pc.field("k") >= v)
-    _same(out, exp)
+    assert_same_table(out, exp)
     m = plan.last_metrics
     assert m["input_batches"] < 8 and m["fast_path_launches"] >= 3, m                                   # pruned row groups never reach the device
     # ScanLimit
-    lim = PL.collect(_scan(path, t.schema, projection=proj, limit=7_500))
-    _same(lim, pq.read_table(path, columns=["f64", "k", "i32"]).slice(0, 7_500))
+    lim = PL.collect(parquet_scan(path, t.schema, projection=proj, limit=7_500))
+    assert_same_table(lim, pq.read_table(path, columns=["f64", "k", "i32"]).slice(0, 7_500))
     # an aggregate straight over the scan: the q1 leaf
     ins = scan.schema()
     g = [E.GroupingExpr("i32", E.Column("i32"))]
     mk = lambda mode, ch: [E.AggExpr("c", mode, PL.create_agg(E.AGG_COUNT, ch, ins, T.int64))]
-    partial = PL.AggExec(PL.HashAgg, g, mk(E.PARTIAL, [E.Column("k")]), False, _scan(path, t.schema, projection=proj))
+    partial = PL.AggExec(PL.HashAgg, g, mk(E.PARTIAL, [E.Column("k")]), False, parquet_scan(path, t.schema, projection=proj))
     final = PL.AggExec(PL.HashAgg, g, mk(E.FINAL, [E.placeholder(T.int64)]), False, partial)
     got = {(r["i32"], r["c"]) for b in PL.collect(final) for r in b.to_pylist()}
     exp = pq.read_table(path, columns=["i32", "k"]).group_by("i32").aggregate([("k", "count")]).to_pylist()
@@ -127,10 +107,10 @@ def test_splits_cover_every_row_group_once_and_missing_columns_are_null(tmp_path
     size = os.path.getsize(path)
     parts = []
     for lo, hi in ((0, size // 3), (size // 3, 2 * size // 3), (2 * size // 3, size)):
-        parts += PL.collect(_scan(path, t.schema, range=(lo, hi)))
-    _same(parts, pq.read_table(path))
+        parts += PL.collect(parquet_scan(path, t.schema, range=(lo, hi)))
+    assert_same_table(parts, pq.read_table(path))
     wider = pa.schema(list(t.schema) + [pa.field("new_col", pa.int64(), True)])                      # schema evolution: the file predates the column
-    out = PL.collect(_scan(path, wider, projection=[0, len(t.schema)]))
+    out = PL.collect(parquet_scan(path, wider, projection=[0, len(t.schema)]))
     got = pa.Table.from_batches(out)
     assert got.column("new_col").null_count == 30_000 and got.column("k").equals(pq.read_table(path).column("k"))
 
@@ -149,12 +129,12 @@ def test_reader_callback_and_unsupported_shapes(tmp_path):
     native.check(native.lib.b200q_set_file_reader(C.cast(reader, C.c_void_p), None))
     try:
         plan = PL.ParquetScanExec(T.from_arrow_schema(t.schema), [("hdfs://nn/warehouse/t.parquet", len(data), None)])
-        _same(PL.collect(plan), pq.read_table(path))
+        assert_same_table(PL.collect(plan), pq.read_table(path))
         assert calls and all(c[0] == "hdfs://nn/warehouse/t.parquet" for c in calls)
     finally:
         native.check(native.lib.b200q_set_file_reader(None, None))
     # zstd pages and string columns are outside the GPU path: UNSUPPORTED, the host keeps its CPU scan
     pq.write_table(t, path, compression="zstd", store_decimal_as_integer=True)
     with pytest.raises(native.NativeError) as ei:
-        PL.collect(_scan(path, t.schema))
+        PL.collect(parquet_scan(path, t.schema))
     assert ei.value.code == native.ERR_UNSUPPORTED
