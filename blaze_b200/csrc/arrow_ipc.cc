@@ -71,7 +71,7 @@ bool next_message(const uint8_t* bytes, size_t n, size_t& cur, Msg& m) {
   return true;
 }
 
-DType parse_field_type(const Table& field) {
+DType parse_field_type(const Table& field, bool allow_binary) {
   uint8_t tt = field.scalar<uint8_t>(2, 0);
   size_t tp = field.indirect(3);
   DType d;
@@ -113,6 +113,7 @@ DType parse_field_type(const Table& field) {
     }
     case TY_Utf8: d.id = T_UTF8; return d;
     case TY_Binary:
+      if (allow_binary) { d.id = T_BINARY; return d; }
       throw PlanError(B200Q_ERR_UNSUPPORTED, "literal: binary literals are not on the hot path");
     default:
       throw PlanError(B200Q_ERR_UNSUPPORTED, "literal: unsupported arrow type tag " + std::to_string(tt));
@@ -121,7 +122,7 @@ DType parse_field_type(const Table& field) {
 
 }  // namespace
 
-ExprP decode_ipc_literal(const uint8_t* bytes, size_t n) {
+ExprP decode_ipc_literal(const uint8_t* bytes, size_t n, bool allow_binary) {
   size_t cur = 0;
   Msg m;
   bool have_schema = false, have_batch = false;
@@ -136,7 +137,7 @@ ExprP decode_ipc_literal(const uint8_t* bytes, size_t n) {
       Vec fields(m.meta, fv);
       if (fields.len < 1) throw PlanError(B200Q_ERR_INVALID_PLAN, "literal: schema without fields");
       size_t f0 = fields.pos + m.meta.rd<uint32_t>(fields.pos);
-      e->type = parse_field_type(Table(m.meta, f0));
+      e->type = parse_field_type(Table(m.meta, f0), allow_binary);
       have_schema = true;
     } else if (m.header_type == HDR_RecordBatch) {
       if (!have_schema) throw PlanError(B200Q_ERR_INVALID_PLAN, "literal: record batch before schema");
@@ -160,11 +161,11 @@ ExprP decode_ipc_literal(const uint8_t* bytes, size_t n) {
       bool valid = true;
       if (null_count > 0) valid = vlen > 0 ? (body[voff] & 1) != 0 : false;
       e->lit_null = !valid;
-      if (valid && e->type.id == T_UTF8) {         // buffers: validity, int32 offsets (row 0: [o0, o1)), data
+      if (valid && e->type.is_varlen()) {          // Utf8 / Binary buffers: validity, int32 offsets (row 0: [o0, o1)), data
         int64_t xoff, xlen; buf_at(2, xoff, xlen);
-        if (dlen < 8) throw PlanError(B200Q_ERR_INVALID_PLAN, "literal: Utf8 offsets buffer too short");
+        if (dlen < 8) throw PlanError(B200Q_ERR_INVALID_PLAN, "literal: " + e->type.str() + " offsets buffer too short");
         int32_t o0, o1; memcpy(&o0, body + doff, 4); memcpy(&o1, body + doff + 4, 4);
-        if (o0 < 0 || o1 < o0 || (int64_t)o1 > xlen) throw PlanError(B200Q_ERR_INVALID_PLAN, "literal: Utf8 offsets out of the data buffer");
+        if (o0 < 0 || o1 < o0 || (int64_t)o1 > xlen) throw PlanError(B200Q_ERR_INVALID_PLAN, "literal: " + e->type.str() + " offsets out of the data buffer");
         e->lit_str.assign((const char*)body + xoff + o0, (size_t)(o1 - o0));
       } else if (valid) {
         const uint8_t* d = body + doff;

@@ -208,7 +208,38 @@ static void build_pipeline(b200q_op* op) {
     last = n;
     if (n->kind == N_FILTER) { for (auto& p : n->predicates) filters.push_back(substitute(p, cur_cols)); pending_tail = true; }
     else if (n->kind == N_PROJECT) { std::vector<ExprP> nc; for (auto& e : n->proj_exprs) nc.push_back(substitute(e, cur_cols)); cur_cols = nc; pending_tail = true; }
-    else if (n->kind == N_AGG) {
+    else if (n->kind == N_AGG && !n->aggs.empty() && n->aggs[0].fn == AGG_BLOOM_FILTER) {
+      // BLOOM_FILTER (decode admits it only without grouping keys and next to other BLOOM_FILTERs): a stage of its own.  Computed
+      // values (the usual XxHash64(col)) and any filter below come from a FilterProjectStage, as trailing columns
+      PlanNode fused;
+      const PlanNode* node = n;
+      if (i + 1 < chain.size() && fusable_partial_final(*n, *chain[i + 1])) {
+        fused = *n; fused.need_final_merge = true; fused.schema = chain[i + 1]->schema;
+        node = &fused; last = chain[i + 1]; i++;
+      }
+      std::vector<int> vcols;
+      SchemaDef bin = stage_in;
+      if (n->need_partial_update) {
+        std::vector<ExprP> vals;
+        bool direct = filters.empty();
+        for (auto& a : n->aggs) {
+          if (a.mode != MODE_PARTIAL) continue;
+          ExprP v = substitute(a.args[0], cur_cols);
+          direct = direct && v->kind == E_COLUMN;
+          vals.push_back(v);
+        }
+        if (direct) for (auto& v : vals) vcols.push_back(v->col_index);
+        else {
+          bin = SchemaDef();
+          for (size_t k = 0; k < vals.size(); k++) { bin.fields.push_back(FieldDef{"#bloom_arg" + std::to_string(k), vals[k]->type, vals[k]->nullable}); vcols.push_back((int)k); }
+          op->stages.push_back(make_filter_project_stage(op->cx, stage_in, filters, vals, bin));
+        }
+      } else if (!filters.empty() || !is_identity(cur_cols, stage_in)) {
+        throw PlanError(B200Q_ERR_UNSUPPORTED, "Filter / Projection fused below a merge-mode BLOOM_FILTER aggregate");
+      }
+      op->stages.push_back(make_bloom_agg_stage(op->cx, bin, *node, vcols));
+      stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in); filters.clear(); pending_tail = false;
+    } else if (n->kind == N_AGG) {
       if (n->need_partial_merge && !is_identity(cur_cols, stage_in)) throw PlanError(B200Q_ERR_UNSUPPORTED, "Projection fused below a merge-mode aggregate");
       push_agg(i, {cur_cols});
     } else if (n->kind == N_EXPAND) {
@@ -222,7 +253,7 @@ static void build_pipeline(b200q_op* op) {
       for (; j < chain.size() && chain[j]->kind == N_PROJECT; j++)
         for (auto& cols : composed) { std::vector<ExprP> nc; for (auto& e : chain[j]->proj_exprs) nc.push_back(substitute(e, cols)); cols = nc; }
       bool fuse = sets.size() > 1 && j < chain.size() && chain[j]->kind == N_AGG && !chain[j]->need_partial_merge;
-      if (fuse) for (auto& a : chain[j]->aggs) fuse = fuse && a.mode == MODE_PARTIAL;
+      if (fuse) for (auto& a : chain[j]->aggs) fuse = fuse && a.mode == MODE_PARTIAL && a.fn != AGG_BLOOM_FILTER;
       if (fuse) { i = j; push_agg(i, composed); continue; }
       op->stages.push_back(make_expand_stage(op->cx, stage_in, filters, sets, n->schema));
       stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in); filters.clear(); pending_tail = false;
@@ -657,6 +688,7 @@ b200q_status b200q_op_create(const uint8_t* plan, size_t plan_len, int32_t plan_
   b200q_op* op = nullptr;
   b200q_status st = guarded(nullptr, [&] {
     PlanP p = decode_plan(plan, plan_len, plan_kind);
+    resolve_scalar_subqueries(*p);           // host work: before the device checks, so its errors do not depend on a GPU
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); throw ExecError(B200Q_ERR_NO_DEVICE, "no CUDA device is visible: the sm_90a kernels cannot run and there is no CPU fallback"); }
     if (device < 0 || device >= ndev) throw ExecError(B200Q_ERR_INVALID_ARG, "invalid device ordinal");
@@ -908,6 +940,7 @@ b200q_status b200q_snappy_uncompress(const uint8_t* src, size_t n, uint8_t* dst,
   });
 }
 b200q_status b200q_set_file_reader(b200q_file_reader_fn fn, void* ctx) { set_file_reader(fn, ctx); return B200Q_OK; }
+b200q_status b200q_set_scalar_subquery_resolver(b200q_scalar_subquery_fn fn, void* ctx) { set_scalar_subquery_resolver((void*)fn, ctx); return B200Q_OK; }
 
 b200q_status b200q_op_attach_build(b200q_op* probe_op, b200q_op* build_op) {
   if (!probe_op || !build_op) return fail(B200Q_ERR_INVALID_ARG, "null argument");

@@ -114,6 +114,7 @@ struct Compiler {
       case E_CASE: return case_(e);
       case E_IN_LIST: return in_list(e);
       case E_SCALAR_FN: return scalar_fn(e);
+      case E_BLOOM: return bloom(e);
       case E_STR_MATCH: {
         expr(e->children[0]);
         emit(VM_LOAD_LIT, 2, 0, str_const(e->lit_str)); push(2);
@@ -272,6 +273,20 @@ struct Compiler {
     return false;
   }
 
+  // BloomFilterMightContain: a NULL filter is `false` for every row without evaluating the value (bloom_filter_might_contain.rs)
+  int bloom(const ExprP& e) {
+    if (!e->bloom) throw PlanError(B200Q_ERR_INVALID_PLAN, "BloomFilterMightContain: the scalar subquery was not resolved");
+    out.vm_only = true;
+    if (e->bloom->is_null) { emit(VM_LOAD_LIT, 0, 0, pool({0, 0})); push(1); return 1; }
+    if (out.blooms.size() >= (size_t)VM_MAX_BLOOMS)
+      throw PlanError(B200Q_ERR_UNSUPPORTED, "more than " + std::to_string(VM_MAX_BLOOMS) + " BloomFilterMightContain expressions in one fused pipeline");
+    expr(e->children[0]);                                        // Int8..Int64: already an i64 on the stack
+    const uint32_t at = pool({0, 64 * (uint64_t)e->bloom->words.size(), (uint64_t)e->bloom->num_hash_functions});
+    out.blooms.push_back(CompiledProgram::BloomRef{at, e->bloom});
+    emit(VM_BLOOM_PROBE, 0, 0, at);
+    return 1;
+  }
+
   int scalar_fn(const ExprP& e) {
     const std::string& nm = e->name;
     if (nm == "Placeholder") throw PlanError(B200Q_ERR_INVALID_PLAN, "placeholder() should never be called");
@@ -296,6 +311,16 @@ struct Compiler {
       emit(VM_NULLIFY, (uint8_t)n); pop(1); return n;
     }
     if (nm == "NormalizeNanAndZero") { expr(e->children[0]); emit(VM_NORM_NAN_ZERO, e->type.id == T_FLOAT32); return 1; }
+    if (nm == "XxHash64") {                 // h = 42; per argument h = xxhash64(value, h), a NULL argument leaves h
+      out.vm_only = true;
+      emit(VM_LOAD_LIT, 0, 0, pool({42, 0})); push(1);
+      for (auto& a : e->children) {
+        if (a->type.id == T_NULL) continue;                      // an untyped NULL hashes nothing
+        const int n = expr(a);
+        emit(VM_XXHASH64, (uint8_t)phys_of(a->type)); pop(n);
+      }
+      return 1;
+    }
     throw PlanError(B200Q_ERR_UNSUPPORTED, "spark ext function '" + nm + "' is not on the hot path");
   }
 };

@@ -14,6 +14,10 @@ struct CompiledProgram {
   std::vector<OutDesc> outs;
   bool has_strings = false;          // reads a Utf8 column or uses a Utf8 constant: only the generic VM kernels run it
   std::vector<uint32_t> str_relocs;  // pool indices holding a str_pool offset, to be turned into a device address at upload
+  bool vm_only = false;              // uses VM_XXHASH64 / VM_BLOOM_PROBE, which only the generic VM kernels implement
+  // bloom filters probed by the program: pool[pool_index] becomes the device address of the uploaded words
+  struct BloomRef { uint32_t pool_index; std::shared_ptr<const BloomFilterDef> filter; };
+  std::vector<BloomRef> blooms;
 };
 
 // filters: conjuncts in evaluation order; outs: projections (FilterExec/ProjectExec kernel) or

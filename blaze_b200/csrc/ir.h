@@ -55,7 +55,7 @@ struct PlanError : std::runtime_error {
 };
 
 enum ExprKind : uint8_t { E_COLUMN, E_LITERAL, E_BINARY, E_IS_NULL, E_IS_NOT_NULL, E_NOT, E_NEGATIVE, E_CAST,
-                          E_TRY_CAST, E_CASE, E_IN_LIST, E_SC_AND, E_SC_OR, E_SCALAR_FN, E_STR_MATCH };
+                          E_TRY_CAST, E_CASE, E_IN_LIST, E_SC_AND, E_SC_OR, E_SCALAR_FN, E_STR_MATCH, E_BLOOM };
 // E_STR_MATCH: StringStartsWith / EndsWith / Contains ExprNode (auron.proto:339-352); pattern in lit_str
 enum StrMatch : uint8_t { SM_STARTS_WITH = 0, SM_ENDS_WITH, SM_CONTAINS };
 enum BinOp : uint8_t { OP_AND, OP_OR, OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE, OP_PLUS, OP_MINUS, OP_MUL, OP_DIV,
@@ -63,6 +63,15 @@ enum BinOp : uint8_t { OP_AND, OP_OR, OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE, 
 
 struct Expr;
 using ExprP = std::shared_ptr<Expr>;
+
+// A Spark bloom filter as SparkBloomFilter::read_from parses it (datafusion-ext-commons/src/spark_bloom_filter.rs): k hash functions
+// over 64 * words.size() bits; `is_null` for a NULL filter value
+struct BloomFilterDef {
+  bool is_null = false;
+  int32_t num_hash_functions = 0;
+  std::vector<uint64_t> words;   // native-endian
+};
+constexpr int VM_MAX_BLOOMS = 4;   // BloomFilterMightContain expressions of one fused program
 
 struct Expr {
   ExprKind kind;
@@ -83,10 +92,14 @@ struct Expr {
   StrMatch str_match = SM_STARTS_WITH;
   // E_CASE: children = [base?] w1 t1 w2 t2 ... [else]; flags say which are present
   bool case_has_base = false, case_has_else = false;
+  // E_BLOOM: BloomFilterMightContain(filter, value); children = {value}, name = uuid.  The filter is `bloom` once known: a Binary
+  // literal is parsed at decode; a scalar-subquery wrapper keeps its serialized bytes in lit_str until op create resolves it
+  std::shared_ptr<const BloomFilterDef> bloom;
+  bool bloom_subquery = false;
   std::vector<ExprP> children;
 };
 
-enum AggFn : uint8_t { AGG_MIN = 0, AGG_MAX = 1, AGG_SUM = 2, AGG_AVG = 3, AGG_COUNT = 4, AGG_FIRST = 7, AGG_FIRST_IGNORES_NULL = 8 };
+enum AggFn : uint8_t { AGG_MIN = 0, AGG_MAX = 1, AGG_SUM = 2, AGG_AVG = 3, AGG_COUNT = 4, AGG_FIRST = 7, AGG_FIRST_IGNORES_NULL = 8, AGG_BLOOM_FILTER = 9 };
 enum AggMode : uint8_t { MODE_PARTIAL = 0, MODE_PARTIAL_MERGE = 1, MODE_FINAL = 2 };
 
 struct AggDef {
@@ -95,6 +108,9 @@ struct AggDef {
   std::string field_name;
   DType data_type;              // Agg::data_type(): Sum/Avg = return_type, Min/Max/First = child type, Count = Int64
   std::vector<ExprP> args;      // after create_agg rewriting: Sum/Avg -> TryCast(child,rt); Count -> nullable children only
+  // BLOOM_FILTER (agg/bloom_filter.rs): the filter a Partial aggregate creates, num_bits bits and k hash functions
+  int64_t bloom_num_bits = 0;
+  int32_t bloom_k = 0;
   bool nullable() const { return fn != AGG_COUNT; }
   DType final_type() const {    // type of the Final-mode output column
     if (fn == AGG_AVG && !data_type.is_decimal()) { DType d; d.id = T_FLOAT64; return d; }
@@ -173,6 +189,8 @@ struct PlanNode {
   bool window_has_limit = false;
   uint32_t window_limit = 0;
   bool output_window_cols = false;
+  // root only: the BloomFilterMightContain expressions whose filter is a scalar subquery (resolved at op create)
+  std::vector<ExprP> subquery_blooms;
 };
 using PlanP = std::shared_ptr<PlanNode>;
 
@@ -191,7 +209,15 @@ std::string explain_plan(const PlanP& p);
 std::string explain_expr(const ExprP& e);
 constexpr const char* AGG_BUF_COLUMN_NAME = "#9223372036854775807";   // agg/mod.rs:37
 
-// arrow_ipc.cc: ScalarValue.ipc_bytes -> literal Expr (auron-serde/src/lib.rs:447-457)
-ExprP decode_ipc_literal(const uint8_t* bytes, size_t n);
+// arrow_ipc.cc: ScalarValue.ipc_bytes -> literal Expr (auron-serde/src/lib.rs:447-457).  Binary literals decode (bytes in lit_str)
+// only where `allow_binary`: the filter argument of BloomFilterMightContain; anywhere else they stay UNSUPPORTED
+ExprP decode_ipc_literal(const uint8_t* bytes, size_t n, bool allow_binary = false);
+
+// plan_decode.cc: SparkBloomFilter::read_from over `n` bytes; malformed bytes -> PlanError(INVALID_ARG) naming the fault
+std::shared_ptr<const BloomFilterDef> parse_spark_bloom_filter(const uint8_t* bytes, size_t n);
+// plan_decode.cc: the process-wide scalar-subquery resolver (b200q_set_scalar_subquery_resolver) and its use at op create: one
+// call per entry of root->subquery_blooms; without a resolver the plan is UNSUPPORTED
+void set_scalar_subquery_resolver(void* fn, void* ctx);
+void resolve_scalar_subqueries(PlanNode& root);
 
 }  // namespace b200q

@@ -1132,10 +1132,7 @@ int launch_ipc_decode_bytes(const IpcCopy* copies, int64_t n, cudaStream_t s) {
 // ---------------------------------------------------------------------------------------------------
 // Spark murmur3 (seed 42) + pmod — hash/mur.rs:19-87, spark_hash.rs:62-200, shuffle/mod.rs:163-188
 // ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t rotl32(uint32_t x, int r) { return (x << r) | (x >> (32 - r)); }
-__device__ __forceinline__ uint32_t mm3_mix_k1(uint32_t k1) { k1 *= 0xcc9e2d51u; k1 = rotl32(k1, 15); k1 *= 0x1b873593u; return k1; }
-__device__ __forceinline__ uint32_t mm3_mix_h1(uint32_t h1, uint32_t k1) { h1 ^= k1; h1 = rotl32(h1, 13); return h1 * 5 + 0xe6546b64u; }
-__device__ __forceinline__ uint32_t mm3_fmix(uint32_t h1, uint32_t len) { h1 ^= len; h1 ^= h1 >> 16; h1 *= 0x85ebca6bu; h1 ^= h1 >> 13; h1 *= 0xc2b2ae35u; h1 ^= h1 >> 16; return h1; }
+// (the murmur3 rounds are in hash.cuh)
 
 struct PhysList { uint8_t phys[VM_MAX_COLS]; };
 

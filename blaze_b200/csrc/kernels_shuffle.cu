@@ -19,17 +19,13 @@
 #include <algorithm>
 #include <cstdlib>
 
+#include "hash.cuh"
 #include "kernels_shuffle.cuh"
 #include "tma.cuh"
 
 namespace b200q {
 
 namespace {
-
-__device__ __forceinline__ uint32_t sh_rotl32(uint32_t x, int r) { return (x << r) | (x >> (32 - r)); }
-__device__ __forceinline__ uint32_t sh_mix_k1(uint32_t k1) { k1 *= 0xcc9e2d51u; k1 = sh_rotl32(k1, 15); k1 *= 0x1b873593u; return k1; }
-__device__ __forceinline__ uint32_t sh_mix_h1(uint32_t h1, uint32_t k1) { h1 ^= k1; h1 = sh_rotl32(h1, 13); return h1 * 5 + 0xe6546b64u; }
-__device__ __forceinline__ uint32_t sh_fmix(uint32_t h1, uint32_t len) { h1 ^= len; h1 ^= h1 >> 16; h1 *= 0x85ebca6bu; h1 ^= h1 >> 13; h1 *= 0xc2b2ae35u; h1 ^= h1 >> 16; return h1; }
 
 int sm_count() {
   int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -61,8 +57,8 @@ __global__ void __launch_bounds__(PID_BLOCK) shuffle_pids_kernel(const ShufSpec 
                    w[0] = (uint32_t)a; w[1] = (uint32_t)(a >> 32); w[2] = (uint32_t)b; w[3] = (uint32_t)(b >> 32); nw = 4; break; }
       }
       uint32_t h1 = h;
-      for (int k = 0; k < nw; k++) h1 = sh_mix_h1(h1, sh_mix_k1(w[k]));
-      h = sh_fmix(h1, (uint32_t)(4 * nw));
+      for (int k = 0; k < nw; k++) h1 = mm3_mix_h1(h1, mm3_mix_k1(w[k]));
+      h = mm3_fmix(h1, (uint32_t)(4 * nw));
     }
     int32_t m = (int32_t)h % P;                                                      // rem_euclid
     if (m < 0) m += P;

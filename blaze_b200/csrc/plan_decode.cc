@@ -6,6 +6,7 @@
 // constructor-time rewrites of `create_agg` (datafusion-ext-plans/src/agg/agg.rs:171-205) and the
 // validation of FilterExec::try_new (filter_exec.rs:58-66) / AggContext::try_new (agg_ctx.rs:110-141).
 // No protoc in this image: the proto3 wire format is read by hand (field numbers cited inline).
+#include <cmath>
 #include <cstring>
 #include <sstream>
 
@@ -230,7 +231,58 @@ ExprP parse_scalar_function(Reader r, const SchemaDef& schema) {   // PhysicalSc
     e->type = args[0]->type; return e;
   }
   if (name == "NormalizeNanAndZero") { if (args.size() != 1 || !args[0]->type.is_float()) bad("NormalizeNanAndZero expects a float"); e->type = args[0]->type; return e; }
+  if (name == "XxHash64") {                 // spark_hash.rs spark_xxhash64: seed 42, chained over the arguments, never NULL
+    if (rt.id != T_INT64) bad("XxHash64 must return int64, not " + rt.str());
+    for (auto& a : args) {
+      const DType& t = a->type;
+      if (!(t.is_intlike() || t.id == T_UTF8 || t.id == T_NULL))
+        unsupported("XxHash64 over a " + t.str() + " argument is not on the hot path");
+    }
+    return e;                               // never NULL, but declared nullable like every ext function (from_proto.rs:965-972)
+  }
   unsupported("spark ext function '" + name + "' is not on the hot path");
+}
+
+// the BloomFilterMightContain expressions of the plan being decoded whose filter is a scalar subquery (decode_plan hands them to the root)
+thread_local std::vector<ExprP>* t_subquery_blooms = nullptr;
+
+// BloomFilterMightContainExprNode{uuid=1, bloom_filter_expr=2, value_expr=3} (auron.proto:357-361; bloom_filter_might_contain.rs).
+// The filter is a Binary literal or a PhysicalSparkScalarSubqueryWrapperExprNode{serialized=1, return_type=2, return_nullable=3}
+// (auron.proto:318-322): the two forms Spark's InjectRuntimeFilter produces.
+ExprP parse_might_contain(Reader r, const SchemaDef& schema) {
+  auto e = mk(E_BLOOM); e->type = bool_t(); e->nullable = true;
+  bool have_filter = false; ExprP value;
+  while (!r.done()) {
+    int wt; uint32_t f = r.tag(wt);
+    if (f == 1) e->name = r.str();
+    else if (f == 2) {
+      Reader x = r.bytes(); have_filter = true;
+      while (!x.done()) {
+        int w; uint32_t g = x.tag(w);
+        if (g == 2) {                        // ScalarValue{ipc_bytes=1}
+          Reader c = x.bytes(); ExprP lit;
+          while (!c.done()) { int w2; uint32_t h = c.tag(w2); if (h == 1) { Reader b = c.bytes(); lit = decode_ipc_literal(b.p, (size_t)(b.end - b.p), true); } else c.skip(w2); }
+          if (!lit) bad("literal without ipc_bytes");
+          if (lit->type.id != T_BINARY && lit->type.id != T_NULL) bad("BloomFilterMightContain: the bloom filter must be a Binary value, not " + lit->type.str());
+          if (lit->lit_null || lit->type.id == T_NULL) { auto d = std::make_shared<BloomFilterDef>(); d->is_null = true; e->bloom = d; }
+          else e->bloom = parse_spark_bloom_filter((const uint8_t*)lit->lit_str.data(), lit->lit_str.size());
+        } else if (g == 10001) {
+          Reader c = x.bytes(); DType rt; bool have_rt = false;
+          while (!c.done()) { int w2; uint32_t h = c.tag(w2); if (h == 1) e->lit_str = c.str(); else if (h == 2) { rt = parse_arrow_type(c.bytes()); have_rt = true; } else c.skip(w2); }
+          if (!have_rt) bad("Missing required field in protobuf");
+          if (rt.id != T_BINARY) bad("BloomFilterMightContain: the scalar subquery must return Binary, not " + rt.str());
+          e->bloom_subquery = true;
+        } else unsupported("BloomFilterMightContain: only a Binary literal or a scalar subquery is on the hot path as the bloom filter");
+      }
+    } else if (f == 3) value = parse_expr(r.bytes(), schema);
+    else r.skip(wt);
+  }
+  if (!have_filter || !value) bad("Missing required field in protobuf");
+  const DType& t = value->type;
+  if (!t.is_integer()) unsupported("BloomFilterMightContain over a " + t.str() + " value is not on the hot path (Int8..Int64 only)");
+  e->children = {value};
+  if (e->bloom_subquery && t_subquery_blooms) t_subquery_blooms->push_back(e);
+  return e;
 }
 
 ExprP parse_expr(Reader r, const SchemaDef& schema) {
@@ -340,7 +392,7 @@ ExprP parse_expr(Reader r, const SchemaDef& schema) {
         e->kind = f == 3000 ? E_SC_AND : E_SC_OR; return e;
       }
       case 20: unsupported("LIKE is not on the hot path");
-      case 10000: case 10001: unsupported("JVM-callback expressions (Spark UDF / scalar subquery wrappers) are not on the hot path");
+      case 10000: case 10001: unsupported("JVM-callback expressions (Spark UDF / scalar subquery wrappers) are not on the hot path outside the bloom filter of BloomFilterMightContain");
       case 10002: case 10003: case 11000: unsupported("nested-type expressions are not on the hot path");
       case 20000: case 20001: case 20002: {   // StringStartsWith/EndsWith/ContainsExprNode{expr=1, prefix|suffix|infix=2} (auron.proto:339-352)
         Reader c = r.bytes(); ExprP x; std::string pat;
@@ -352,7 +404,7 @@ ExprP parse_expr(Reader r, const SchemaDef& schema) {
         return e;
       }
       case 20100: unsupported("RowNum is not on the hot path");
-      case 20200: unsupported("BloomFilterMightContain is not on the hot path");
+      case 20200: return parse_might_contain(r.bytes(), schema);
       default: r.skip(wt);
     }
   }
@@ -546,11 +598,33 @@ PlanP parse_agg(Reader r) {                  // AggExecNode (auron.proto:675-685
     if (!have_rt) bad("Missing required field in protobuf");
     if (modes[i] > 2) bad("invalid AggMode");
     a.mode = (AggMode)modes[i]; a.field_name = anames[i];
-    if (fn > 4 && fn != AGG_FIRST && fn != AGG_FIRST_IGNORES_NULL)
+    if (fn > 4 && fn != AGG_FIRST && fn != AGG_FIRST_IGNORES_NULL && fn != AGG_BLOOM_FILTER)
       unsupported("aggregate function #" + std::to_string(fn) + " is out of the hot-path scope (variable-length / JVM-callback state)");
     a.fn = (AggFn)fn;
-    // create_agg (agg/agg.rs:171-213)
-    if (a.fn == AGG_FIRST || a.fn == AGG_FIRST_IGNORES_NULL) {
+    // create_agg (agg/agg.rs:171-232)
+    if (a.fn == AGG_BLOOM_FILTER) {
+      if (!n->group_exprs.empty()) unsupported("aggregate function #9 (BLOOM_FILTER) with grouping keys is not on the hot path");
+      // children: value, literal estimated_num_items, literal num_bits (agg.rs:214-232; AggBloomFilter::new asserts a power of two)
+      if (children.size() != 3) bad("BLOOM_FILTER expects 3 children (value, estimated_num_items, num_bits), got " + std::to_string(children.size()));
+      auto lit_i64 = [&](size_t i, const char* what) {
+        const ExprP& c = children[i];
+        if (c->kind != E_LITERAL || c->lit_null || !c->type.is_integer()) bad(std::string("BLOOM_FILTER: ") + what + " must be a non-NULL integer literal");
+        return (int64_t)c->lit_lo;
+      };
+      const int64_t est = lit_i64(1, "estimated_num_items"), bits = lit_i64(2, "num_bits");
+      if (bits <= 0 || (bits & (bits - 1)) != 0) bad("BLOOM_FILTER: num_bits " + std::to_string(bits) + " is not a power of two");
+      if (bits > 0x7FFFFFFF) bad("BLOOM_FILTER: num_bits " + std::to_string(bits) + " exceeds INT32_MAX");
+      if (est <= 0) bad("BLOOM_FILTER: estimated_num_items " + std::to_string(est) + " is not positive");
+      a.bloom_num_bits = bits;
+      const double kk = std::round((double)bits / (double)est * std::log(2.0));     // optimal_num_of_hash_functions
+      a.bloom_k = (int32_t)std::max(1.0, std::min(kk, 2147483647.0));
+      a.data_type.id = T_BINARY;
+      const DType& vt = children[0]->type;
+      if (a.mode == MODE_PARTIAL) {
+        if (!vt.is_integer()) unsupported("BLOOM_FILTER over a " + vt.str() + " value is not on the hot path (Int8..Int64 only)");
+        a.args.push_back(children[0]);
+      }
+    } else if (a.fn == AGG_FIRST || a.fn == AGG_FIRST_IGNORES_NULL) {
       if (children.empty()) bad("aggregate without children");
       // the child's type; a merge-side Placeholder has the Null type, so the state type comes from return_type
       a.data_type = children[0]->type.id == T_NULL ? rt : children[0]->type;
@@ -579,6 +653,9 @@ PlanP parse_agg(Reader r) {                  // AggExecNode (auron.proto:675-685
     }
     n->aggs.push_back(a);
   }
+  size_t n_bloom = 0;
+  for (auto& a : n->aggs) n_bloom += a.fn == AGG_BLOOM_FILTER;
+  if (n_bloom && n_bloom != n->aggs.size()) unsupported("aggregate function #9 (BLOOM_FILTER) next to other aggregates in one AggExec is not on the hot path");
   for (auto& a : n->aggs) {
     n->need_partial_update |= a.mode == MODE_PARTIAL;
     n->need_partial_merge |= a.mode != MODE_PARTIAL;
@@ -965,6 +1042,13 @@ std::string explain_expr(const ExprP& e) {
     case E_IN_LIST: { o << explain_expr(e->children[0]) << (e->negated ? " NOT IN (" : " IN ("); for (size_t i = 1; i < e->children.size(); i++) o << (i > 1 ? ", " : "") << explain_expr(e->children[i]); o << ")"; break; }
     case E_STR_MATCH: { static const char* nm[] = {"StartsWith", "EndsWith", "Contains"}; o << nm[e->str_match] << "(" << explain_expr(e->children[0]) << ", '" << e->lit_str << "')"; break; }
     case E_SCALAR_FN: { o << e->name << "("; for (size_t i = 0; i < e->children.size(); i++) o << (i ? ", " : "") << explain_expr(e->children[i]); o << ")"; break; }
+    case E_BLOOM: {
+      o << "BloomFilterMightContain(uuid=" << e->name << ", ";
+      if (e->bloom_subquery && !e->bloom) o << "ScalarSubquery(" << e->lit_str.size() << " bytes)";
+      else if (e->bloom->is_null) o << "NULL:binary";
+      else o << "SparkBloomFilter(k=" << e->bloom->num_hash_functions << ", bits=" << 64 * e->bloom->words.size() << ")";
+      o << ", " << explain_expr(e->children[0]) << ")"; break;
+    }
   }
   return o.str();
 }
@@ -996,7 +1080,7 @@ static void explain_rec(const PlanP& p, int depth, std::ostringstream& o) {
       for (size_t i = 0; i < p->proj_exprs.size(); i++) o << (i ? ", " : "") << explain_expr(p->proj_exprs[i]) << " AS " << p->schema.fields[i].name;
       o << "] schema=" << schema_str(p->schema) << "\n"; break;
     case N_AGG: {
-      static const char* fn[] = {"Min", "Max", "Sum", "Avg", "Count", "CollectList", "CollectSet", "First", "FirstIgnoresNull"};
+      static const char* fn[] = {"Min", "Max", "Sum", "Avg", "Count", "CollectList", "CollectSet", "First", "FirstIgnoresNull", "BloomFilter"};
       static const char* md[] = {"Partial", "PartialMerge", "Final"};
       o << ind << "AggExec " << (p->exec_mode == 0 ? "HashAgg" : "SortAgg") << " groupings=[";
       for (size_t i = 0; i < p->group_exprs.size(); i++) o << (i ? ", " : "") << explain_expr(p->group_exprs[i]) << " AS " << p->group_names[i];
@@ -1004,7 +1088,9 @@ static void explain_rec(const PlanP& p, int depth, std::ostringstream& o) {
       for (size_t i = 0; i < p->aggs.size(); i++) {
         auto& a = p->aggs[i]; o << (i ? ", " : "") << fn[a.fn] << "(";
         for (size_t j = 0; j < a.args.size(); j++) o << (j ? ", " : "") << explain_expr(a.args[j]);
-        o << "):" << a.data_type.str() << "/" << md[a.mode] << " AS " << a.field_name;
+        o << ")";
+        if (a.fn == AGG_BLOOM_FILTER) o << "[num_bits=" << a.bloom_num_bits << ", k=" << a.bloom_k << "]";
+        o << ":" << a.data_type.str() << "/" << md[a.mode] << " AS " << a.field_name;
       }
       o << "] partial_skipping=" << (p->supports_partial_skipping ? "true" : "false") << " schema=" << schema_str(p->schema) << "\n"; break;
     }
@@ -1083,14 +1169,71 @@ std::string explain_plan(const PlanP& p) { std::ostringstream o; explain_rec(p, 
 PlanP decode_plan(const uint8_t* bytes, size_t n, int plan_kind) {
   if (!bytes && n) bad("null plan bytes");
   Reader r(bytes, n);
+  std::vector<ExprP> subquery_blooms;
+  struct Collect {                          // restores the collector on every exit, exceptions included
+    std::vector<ExprP>* prev;
+    explicit Collect(std::vector<ExprP>* v) : prev(t_subquery_blooms) { t_subquery_blooms = v; }
+    ~Collect() { t_subquery_blooms = prev; }
+  } collect(&subquery_blooms);
+  PlanP p;
   if (plan_kind == B200Q_TASK_DEFINITION) {   // TaskDefinition{task_id=1, plan=2, output_partitioning=3}
-    PlanP p;
     while (!r.done()) { int wt; uint32_t f = r.tag(wt); if (f == 2) p = parse_plan(r.bytes()); else r.skip(wt); }
     if (!p) bad("TaskDefinition without plan");
-    return p;
+  } else {
+    if (plan_kind != B200Q_PLAN_NODE) throw PlanError(B200Q_ERR_INVALID_ARG, "unknown plan_kind");
+    p = parse_plan(r);
   }
-  if (plan_kind != B200Q_PLAN_NODE) throw PlanError(B200Q_ERR_INVALID_ARG, "unknown plan_kind");
-  return parse_plan(r);
+  p->subquery_blooms = std::move(subquery_blooms);
+  return p;
+}
+
+// SparkBloomFilter::read_from + SparkBitArray::read_from (spark_bloom_filter.rs, spark_bit_array.rs): big-endian i32 version (1),
+// i32 num_hash_functions, i32 num_words, then num_words big-endian i64 words.  The reference reads whatever is there; here every
+// field is checked, so that a corrupt filter is an error instead of a probe outside the bit array.
+std::shared_ptr<const BloomFilterDef> parse_spark_bloom_filter(const uint8_t* b, size_t n) {
+  auto fault = [](const std::string& m) { throw PlanError(B200Q_ERR_INVALID_ARG, "bloom filter: " + m); };
+  auto be32 = [&](size_t at) { return (int32_t)((uint32_t)b[at] << 24 | (uint32_t)b[at + 1] << 16 | (uint32_t)b[at + 2] << 8 | (uint32_t)b[at + 3]); };
+  if (n < 12) fault(std::to_string(n) + " bytes, shorter than the 12-byte header");
+  const int32_t version = be32(0), k = be32(4), words = be32(8);
+  if (version != 1) fault("unsupported version " + std::to_string(version) + " (expected 1)");
+  if (k <= 0) fault("num_hash_functions " + std::to_string(k) + " is not positive");
+  if (words <= 0) fault("num_words " + std::to_string(words) + " is not positive");
+  if ((int64_t)words * 64 > 0x7FFFFFFF) fault("num_words " + std::to_string(words) + " makes more than INT32_MAX bits");
+  const size_t want = 12 + 8 * (size_t)words;
+  if (n != want) fault(std::to_string(n) + " bytes where num_words " + std::to_string(words) + " needs " + std::to_string(want));
+  auto d = std::make_shared<BloomFilterDef>();
+  d->num_hash_functions = k;
+  d->words.resize((size_t)words);
+  for (size_t i = 0; i < (size_t)words; i++) {
+    uint64_t v = 0;
+    for (int j = 0; j < 8; j++) v = v << 8 | b[12 + 8 * i + j];
+    d->words[i] = v;
+  }
+  return d;
+}
+
+namespace {
+b200q_scalar_subquery_fn g_subquery_fn = nullptr;
+void* g_subquery_ctx = nullptr;
+struct SubquerySink { std::string value; bool put = false; };
+void subquery_put(void* sink, const uint8_t* data, size_t len) {   // the library copies the bytes before it returns
+  auto* k = static_cast<SubquerySink*>(sink);
+  k->value.assign((const char*)data, data ? len : 0); k->put = true;
+}
+}  // namespace
+
+void set_scalar_subquery_resolver(void* fn, void* ctx) { g_subquery_fn = (b200q_scalar_subquery_fn)fn; g_subquery_ctx = ctx; }
+
+void resolve_scalar_subqueries(PlanNode& root) {
+  if (root.subquery_blooms.empty()) return;
+  if (!g_subquery_fn) unsupported("BloomFilterMightContain: the scalar subquery needs a resolver (b200q_set_scalar_subquery_resolver)");
+  for (auto& e : root.subquery_blooms) {
+    SubquerySink sink;
+    const int32_t st = g_subquery_fn(g_subquery_ctx, (const uint8_t*)e->lit_str.data(), e->lit_str.size(), subquery_put, &sink);
+    if (st != 0) throw PlanError(B200Q_ERR_EXECUTION, "BloomFilterMightContain: the scalar subquery resolver failed with status " + std::to_string(st));
+    if (!sink.put) { auto d = std::make_shared<BloomFilterDef>(); d->is_null = true; e->bloom = d; }      // NULL: false for every row
+    else e->bloom = parse_spark_bloom_filter((const uint8_t*)sink.value.data(), sink.value.size());
+  }
 }
 
 }  // namespace b200q

@@ -109,6 +109,10 @@ std::unique_ptr<Stage> make_agg_stage(OpContext& cx, const SchemaDef& in_schema,
                                       const std::vector<ExprP>& group_exprs, const std::vector<std::vector<ExprP>>& agg_args,
                                       const std::vector<AggSetExprs>& sets = {});
 
+// AggExec whose aggregates are all BLOOM_FILTER, without grouping keys (bloom_stage.cu).  Partial: value_cols[i] is the input
+// column of aggregate i's value; merge modes read the Binary state column(s) of the input
+std::unique_ptr<Stage> make_bloom_agg_stage(OpContext& cx, const SchemaDef& in_schema, const PlanNode& agg, const std::vector<int>& value_cols);
+
 // ShuffleWriterExec (shuffle_stage.cu): terminal stage; its result is the two shuffle files and/or the encoded chunks
 std::unique_ptr<Stage> make_shuffle_write_stage(OpContext& cx, const SchemaDef& in_schema, const PlanNode& node);
 struct ShuffleResult {

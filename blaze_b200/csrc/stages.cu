@@ -136,10 +136,18 @@ void add_kernel_time(OpContext& cx, int64_t rows, bool hot) {
   if (hot) { cx.m.hot_ms += ms; cx.m.hot_rows += rows; cx.m.hot_launches++; }
 }
 
-// the program in device memory, its Utf8 constants relocated to their device addresses
-static DevMemP upload_program(const CompiledProgram& cp, cudaStream_t s) {
+// the program in device memory, its Utf8 constants relocated to their device addresses; the bit words of its bloom filters go to
+// `blooms`, which the stage keeps as long as the program
+static DevMemP upload_program(const CompiledProgram& cp, cudaStream_t s, std::vector<DevMemP>& blooms) {
   DevMemP d = DevMem::alloc(sizeof(VmProgram), s);
-  const VmProgram p = relocated_program(cp, d->ptr);
+  VmProgram p = relocated_program(cp, d->ptr);
+  for (const auto& b : cp.blooms) {
+    const size_t bytes = b.filter->words.size() * 8;
+    DevMemP w = DevMem::alloc(bytes, s);
+    B200Q_CUDA(cudaMemcpyAsync(w->ptr, b.filter->words.data(), bytes, cudaMemcpyHostToDevice, s));
+    p.pool[b.pool_index] = (uint64_t)(uintptr_t)w->ptr;
+    blooms.push_back(w);
+  }
   B200Q_CUDA(cudaMemcpyAsync(d->ptr, &p, sizeof(VmProgram), cudaMemcpyHostToDevice, s));
   B200Q_CUDA(cudaStreamSynchronize(s));                 // `p` lives on this stack frame
   return d;
@@ -157,6 +165,7 @@ static void check_device_error_flags(int flags) {
 class FilterProjectStage : public Stage {
   CompiledProgram cp_;
   DevMemP d_prog_;
+  std::vector<DevMemP> d_blooms_;    // bit words of the program's bloom filters
   bool has_filters_;
   bool identity_ = false;            // no filter, output i = input column i: batches are forwarded as they are (no copy, no launch)
   bool lean_possible_ = false;
@@ -220,8 +229,8 @@ class FilterProjectStage : public Stage {
     cp_ = compile_program(filters, vm_outs, has_filters_, sel_out_);
     used_input_cols = cp_.used_cols;
     for (int c : out_src_) if (c >= 0 && std::find(used_input_cols.begin(), used_input_cols.end(), c) == used_input_cols.end()) used_input_cols.push_back(c);
-    if (!cx.conf.force_generic_kernels && !varlen_ && !cp_.has_strings) detect_lean(filters, outs);
-    d_prog_ = upload_program(cp_, cx.stream);
+    if (!cx.conf.force_generic_kernels && !varlen_ && !cp_.has_strings && !cp_.vm_only) detect_lean(filters, outs);
+    d_prog_ = upload_program(cp_, cx.stream, d_blooms_);
   }
 
   void push(OpContext& cx, DevBatch& in, std::vector<DevBatch>& outs) override {
@@ -407,6 +416,7 @@ static bool same_expr(const ExprP& a, const ExprP& b) {
   if (a->kind == E_STR_MATCH && (a->str_match != b->str_match || a->lit_str != b->lit_str)) return false;
   if (a->kind == E_BINARY && a->op != b->op) return false;
   if (a->kind == E_SCALAR_FN && a->name != b->name) return false;
+  if (a->kind == E_BLOOM && a->bloom != b->bloom) return false;            // the same value probed in two filters
   if (a->kind == E_IN_LIST && a->negated != b->negated) return false;
   if (a->kind == E_CASE && (a->case_has_base != b->case_has_base || a->case_has_else != b->case_has_else)) return false;
   for (size_t i = 0; i < a->children.size(); i++) if (!same_expr(a->children[i], b->children[i])) return false;
@@ -462,6 +472,7 @@ class AggStage : public Stage {
   std::vector<ExprP> vm_outs_;          // keys, then accumulator arguments
   CompiledProgram cp_;
   DevMemP d_prog_;
+  std::vector<DevMemP> d_blooms_;       // bit words of the program's bloom filters
   AggLayout lay_{};
   bool merge_mode_ = false, columnar_ = false, final_ = false;
   int n_in_ = 0;                        // input columns
@@ -783,14 +794,15 @@ class AggStage : public Stage {
     if (merge_mode_ && !columnar_) used_input_cols.push_back(n_in_ - 1);
     std::sort(used_input_cols.begin(), used_input_cols.end());
     used_input_cols.erase(std::unique(used_input_cols.begin(), used_input_cols.end()), used_input_cols.end());
-    d_prog_ = upload_program(cp_, cx.stream);
+    d_prog_ = upload_program(cp_, cx.stream, d_blooms_);
     if (multi) {                              // the set descriptors travel next to the program (they do not fit the kernel parameters)
       d_sets_ = DevMem::alloc(sizeof(AggSetDesc) * sets_.size(), cx.stream);
       B200Q_CUDA(cudaMemcpyAsync(d_sets_->ptr, sets_.data(), sizeof(AggSetDesc) * sets_.size(), cudaMemcpyHostToDevice, cx.stream));
     }
 
-    if (!cp_.has_strings && !multi) {         // the specialised kernels read fixed-width columns only: string programs stay on the VM kernel;
-                                              // they insert one key per row, so grouping sets stay on the VM kernel too
+    if (!cp_.has_strings && !cp_.vm_only && !multi) {   // the specialised kernels read fixed-width columns only: string programs stay on
+                                              // the VM kernel, as do XxHash64 / bloom probes, which only the VM implements; they insert
+                                              // one key per row, so grouping sets stay on the VM kernel too
       detect_fast(cx);
       if (!fast_ok_) detect_wide(cx);
     }

@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "hash.cuh"
 #include "vm.h"
 
 namespace b200q {
@@ -171,6 +172,45 @@ __device__ __forceinline__ int vm_str(const VmInstr in, const uint64_t* __restri
       return ix + 1;
     }
   }
+}
+
+// VM_XXHASH64 (spark_hash.rs create_xxhash64_hashes: Bool / Int8 / Int16 / Int32 / Date32 hash as a 4-byte int, Int64 /
+// Timestamp as an 8-byte long, Utf8 over its bytes) and VM_BLOOM_PROBE (SparkBloomFilter::might_contain_long).  Returns the new
+// stack pointer.
+template <int R>
+__device__ __forceinline__ int vm_bloom(const VmInstr in, const uint64_t* __restrict__ pool, uint64_t (&st)[VM_MAX_DEPTH][R], uint32_t (&vm)[R], int sp) {
+  if (in.op == VM_XXHASH64) {
+    const int is = sp - (in.a == PH_STR ? 3 : 2);   // the seed; the value above it
+    FORR {
+      uint64_t h = st[is][r];
+      if (VALID(r, is + 1)) {
+        const uint64_t v = st[is + 1][r];
+        if (in.a == PH_STR) h = xxh64_bytes(STRP(v), (uint32_t)st[is + 2][r], h);
+        else if (in.a == PH_I64) h = xxh64_long(v, h);
+        else h = xxh64_int((uint32_t)v, h);
+      }
+      st[is][r] = h;
+    }
+    return is + 1;
+  }
+  const uint64_t* __restrict__ bits = (const uint64_t*)(uintptr_t)pool[in.c];
+  const int32_t bit_size = (int32_t)pool[in.c + 1], k = (int32_t)pool[in.c + 2];
+  FORR {
+    bool v = false;
+    if (VALID(r, sp - 1)) {
+      const int64_t x = (int64_t)st[sp - 1][r];
+      const int32_t h1 = mm3_hash_long(x, 0), h2 = mm3_hash_long(x, h1);
+      v = true;
+      for (int32_t i = 1; i <= k && v; i++) {
+        int32_t c = (int32_t)((uint32_t)h1 + (uint32_t)i * (uint32_t)h2);   // i32 wrapping
+        if (c < 0) c = ~c;                                                  // flip all bits if negative
+        const uint32_t b = (uint32_t)(c % bit_size);
+        v = (__ldg(bits + (b >> 6)) >> (b & 63)) & 1;
+      }
+    }
+    st[sp - 1][r] = v;
+  }
+  return sp;
 }
 
 // Runs from `pc` until VM_END (returns -1) or VM_COMPACT (returns the pc after it).
@@ -512,6 +552,7 @@ __device__ __forceinline__ int vm_run(const VmInstr* __restrict__ code, const ui
       }
       case VM_OUT_SEL: FORR { sink.out(r, (int)in.b, (int)PH_SEL, (uint64_t)row[r], 0ULL, true); } break;
       case VM_CMP_STR: case VM_STARTS_WITH: case VM_ENDS_WITH: case VM_CONTAINS: case VM_CAST_STR_I: sp = vm_str<R>(in, pool, st, vm, sp); break;
+      case VM_XXHASH64: case VM_BLOOM_PROBE: sp = vm_bloom<R>(in, pool, st, vm, sp); break;
       default: return -1;
     }
   }

@@ -51,6 +51,9 @@ enum VmOp : uint8_t {
   VM_CAST_STR_I,      // a = target bits: Spark UTF8String.toLong/toInt (commons cast.rs:287-361); NULL on bad input
   VM_LOAD_STR,        // b = column slot: pushes {pointer into the data, length} of a Utf8 column
   VM_OUT_SEL,         // b = output index: the source row of the (surviving) row, for the variable-width gathers
+  // Spark's runtime bloom filters (only the generic VM kernels run programs that use these)
+  VM_XXHASH64,        // a = PhysKind of the operand: pops value, i64 seed -> xxhash64(value, seed); a NULL value leaves the seed
+  VM_BLOOM_PROBE,     // c = pool{device address of the bit words, bit size, k}: pops an i64 -> might_contain_long; NULL stays NULL
 };
 
 enum PhysKind : uint8_t { PH_BOOL = 0, PH_I8, PH_I16, PH_I32, PH_I64, PH_F32, PH_F64, PH_DEC128, PH_STR,

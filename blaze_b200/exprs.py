@@ -262,7 +262,7 @@ def Contains(expr: Expr, infix: str) -> StringMatch: return StringMatch("Contain
 
 # Spark ext functions on the hot path (datafusion-ext-functions/src/lib.rs:34-68)
 SPARK_EXT_FUNCTIONS = ("UnscaledValue", "MakeDecimal", "CheckOverflow", "NullIfZero", "NullIf",
-                       "NormalizeNanAndZero", "Placeholder")
+                       "NormalizeNanAndZero", "Placeholder", "XxHash64")
 
 
 @dataclass(frozen=True)
@@ -283,13 +283,47 @@ class ScalarFunction(Expr):
     def nullable(self, schema): return True
 
 
+def XxHash64(*args: Expr) -> ScalarFunction:
+    """Spark's XxHash64(children, 42) (spark_hash.rs spark_xxhash64): h = 42, then h = xxhash64(child, h) per child; a NULL
+    child leaves h unchanged, so the result is never NULL."""
+    return ScalarFunction("XxHash64", args, T.int64)
+
+
+@dataclass(frozen=True)
+class ScalarSubquery(Expr):
+    """`PhysicalSparkScalarSubqueryWrapperExprNode{serialized, return_type, return_nullable}` (auron.proto:318-322): a scalar
+    subquery the JVM evaluates.  On the device path it is accepted only as the bloom filter of BloomFilterMightContain, and
+    the host's resolver (native.set_scalar_subquery_resolver) turns `serialized` into the value at op create."""
+    serialized: bytes
+    return_type: DataType = T.binary
+    return_nullable: bool = True
+
+    def data_type(self, schema): return self.return_type
+    def nullable(self, schema): return self.return_nullable
+
+
+@dataclass(frozen=True)
+class BloomFilterMightContain(Expr):
+    """`BloomFilterMightContainExprNode{uuid, bloom_filter_expr, value_expr}` (bloom_filter_might_contain.rs): whether the
+    Spark bloom filter (a Binary literal, or a ScalarSubquery) might contain the Int8..Int64 value.  A NULL filter gives false
+    for every row; a NULL value gives NULL."""
+    bloom_filter: Expr
+    value: Expr
+    uuid: str = ""
+
+    def children(self): return (self.bloom_filter, self.value)
+    def data_type(self, schema): return T.bool_
+    def nullable(self, schema): return True
+
+
 # ---- aggregate descriptions ----------------------------------------------------------------------
 
 # AggFunction enum values (auron.proto:127-141)
 AGG_MIN, AGG_MAX, AGG_SUM, AGG_AVG, AGG_COUNT = 0, 1, 2, 3, 4
 AGG_FIRST, AGG_FIRST_IGNORES_NULL = 7, 8
+AGG_BLOOM_FILTER = 9             # children: value, Literal(estimated_num_items), Literal(num_bits); the state and result are Binary
 AGG_NAMES = {AGG_MIN: "Min", AGG_MAX: "Max", AGG_SUM: "Sum", AGG_AVG: "Avg", AGG_COUNT: "Count",
-             AGG_FIRST: "First", AGG_FIRST_IGNORES_NULL: "FirstIgnoresNull"}
+             AGG_FIRST: "First", AGG_FIRST_IGNORES_NULL: "FirstIgnoresNull", AGG_BLOOM_FILTER: "BloomFilter"}
 
 # AggMode (auron.proto:692-696) / AggExecMode (:687-690)
 PARTIAL, PARTIAL_MERGE, FINAL = 0, 1, 2

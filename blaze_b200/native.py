@@ -77,7 +77,7 @@ SYMBOLS = ["b200q_version", "b200q_build_info", "b200q_last_error", "b200q_devic
            "b200q_op_push_device", "b200q_op_finish", "b200q_op_pull", "b200q_op_pull_device", "b200q_op_sync",
            "b200q_op_metrics", "b200q_op_destroy", "b200q_murmur3_partition",
            "b200q_set_file_reader", "b200q_parquet_explain", "b200q_snappy_uncompress", "b200q_op_attach_build", "b200q_op_attach_right", "b200q_op_shuffle_chunk_count", "b200q_op_shuffle_chunk", "b200q_lz4_frame_compress",
-           "b200q_lz4_frame_decompress", "b200q_op_push_ipc",
+           "b200q_lz4_frame_decompress", "b200q_op_push_ipc", "b200q_set_scalar_subquery_resolver",
            "b200q_exchange_unique_id", "b200q_exchange_create", "b200q_exchange_shuffle", "b200q_exchange_kernel_launches",
            "b200q_exchange_destroy"]
 
@@ -116,6 +116,7 @@ def _load():
     lib.b200q_lz4_frame_compress.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.b200q_lz4_frame_decompress.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.b200q_op_push_ipc.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]
+    lib.b200q_set_scalar_subquery_resolver.argtypes = [C.c_void_p, C.c_void_p]
     lib.b200q_exchange_unique_id.argtypes = [C.c_void_p]
     lib.b200q_exchange_create.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
     lib.b200q_exchange_shuffle.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
@@ -163,6 +164,36 @@ def lz4_frame_decompress(data: bytes) -> bytes:
     buf = C.create_string_buffer(max(1, need.value))
     check(lib.b200q_lz4_frame_decompress(data, len(data), buf, need.value, C.byref(need)))
     return buf.raw[: need.value]
+
+
+_BYTES_SINK = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_size_t)
+_SUBQUERY_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.POINTER(C.c_uint8), C.c_size_t, C.c_void_p, C.c_void_p)
+_resolver_keepalive = None
+
+
+def set_scalar_subquery_resolver(fn) -> None:
+    """Register `fn(serialized: bytes) -> bytes | None` as the process-wide scalar-subquery resolver
+    (b200q_set_scalar_subquery_resolver): op create calls it once per BloomFilterMightContain whose filter is a ScalarSubquery.
+    None removes it.  An exception raised by `fn` fails the create with ERR_EXECUTION."""
+    global _resolver_keepalive
+    if fn is None:
+        check(lib.b200q_set_scalar_subquery_resolver(None, None))
+        _resolver_keepalive = None
+        return
+
+    def trampoline(_ctx, serialized, n, put, sink):
+        try:
+            v = fn(C.string_at(serialized, n) if n else b"")
+        except Exception:
+            return 1
+        if v is not None:
+            v = bytes(v)
+            _BYTES_SINK(put)(sink, C.cast(C.c_char_p(v), C.c_void_p), len(v))
+        return 0
+
+    cb = _SUBQUERY_FN(trampoline)
+    check(lib.b200q_set_scalar_subquery_resolver(C.cast(cb, C.c_void_p), None))
+    _resolver_keepalive = cb                    # the library holds the pointer: keep the ctypes thunk alive
 
 
 def last_error() -> str:

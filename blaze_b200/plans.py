@@ -457,6 +457,8 @@ class ShuffleWriterExec(ExecutionPlan):
 def _agg_data_type(f: AggFunctionExpr, ins: Schema) -> T.DataType:
     if f.function == E.AGG_COUNT:
         return T.int64
+    if f.function == E.AGG_BLOOM_FILTER:
+        return T.binary                                                                               # bloom_filter.rs data_type
     if f.function in (E.AGG_SUM, E.AGG_AVG):
         return f.return_type
     dt = f.children[0].data_type(ins)

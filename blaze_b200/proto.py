@@ -115,6 +115,8 @@ def _build_pool():
         ("negative", 12, "PhysicalNegativeNode", O), ("in_list", 13, "PhysicalInListNode", O),
         ("scalar_function", 14, "PhysicalScalarFunctionNode", O), ("try_cast", 15, "PhysicalTryCastNode", O),
         ("sc_and_expr", 3000, "PhysicalSCAndExprNode", O), ("sc_or_expr", 3001, "PhysicalSCOrExprNode", O),
+        ("spark_scalar_subquery_wrapper_expr", 10001, "PhysicalExprNode.PhysicalSparkScalarSubqueryWrapperExprNode", O),
+        ("bloom_filter_might_contain_expr", 20200, "PhysicalExprNode.BloomFilterMightContainExprNode", O),
         ("string_starts_with_expr", 20000, "PhysicalExprNode.StringStartsWithExprNode", O),
         ("string_ends_with_expr", 20001, "PhysicalExprNode.StringEndsWithExprNode", O),
         ("string_contains_expr", 20002, "PhysicalExprNode.StringContainsExprNode", O),
@@ -133,6 +135,14 @@ def _build_pool():
                 f.type, f.type_name = _F.TYPE_MESSAGE, f".{_PKG}.{typ}"
             else:
                 f.type = typ
+
+    # PhysicalSparkScalarSubqueryWrapperExprNode{serialized=1, return_type=2, return_nullable=3} and BloomFilterMightContainExprNode
+    # {uuid=1, bloom_filter_expr=2, value_expr=3} (auron.proto:318-322, 357-361): nested the same way; tests/test_bloom_host.py checks
+    # their fields against tests/golden/auron_proto_bloom_fields.json
+    _msg(fd, "PhysicalSparkScalarSubqueryWrapperExprNode", [("serialized", 1, _F.TYPE_BYTES), ("return_type", 2, "ArrowType"),
+                                                             ("return_nullable", 3, _F.TYPE_BOOL)], into=px.nested_type)
+    _msg(fd, "BloomFilterMightContainExprNode", [("uuid", 1, _F.TYPE_STRING), ("bloom_filter_expr", 2, "PhysicalExprNode"),
+                                                  ("value_expr", 3, "PhysicalExprNode")], into=px.nested_type)
 
     _msg(fd, "FilterExecNode", [("input", 1, "PhysicalPlanNode"), ("expr", 2, "PhysicalExprNode", R)])
     _msg(fd, "ProjectionExecNode", [("input", 1, "PhysicalPlanNode"), ("expr", 2, "PhysicalExprNode", R),
@@ -343,6 +353,16 @@ def expr_msg(e: E.Expr):
         sm = getattr(m, field)
         sm.expr.CopyFrom(expr_msg(e.expr))
         setattr(sm, pat, e.pattern)
+    elif isinstance(e, E.ScalarSubquery):
+        w = m.spark_scalar_subquery_wrapper_expr
+        w.serialized = e.serialized
+        w.return_type.CopyFrom(arrow_type_msg(e.return_type))
+        w.return_nullable = e.return_nullable
+    elif isinstance(e, E.BloomFilterMightContain):
+        b = m.bloom_filter_might_contain_expr
+        b.uuid = e.uuid
+        b.bloom_filter_expr.CopyFrom(expr_msg(e.bloom_filter))
+        b.value_expr.CopyFrom(expr_msg(e.value))
     elif isinstance(e, E.ScalarFunction):
         sf = m.scalar_function
         sf.name = e.name

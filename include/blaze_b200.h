@@ -266,6 +266,18 @@ b200q_status b200q_op_attach_right(b200q_op* join_op, b200q_op* right_op);
  * [offset, offset + length) of `path` and return 0. */
 typedef int32_t (*b200q_file_reader_fn)(void* ctx, const char* path, int64_t offset, int64_t length, uint8_t* dst);
 b200q_status b200q_set_file_reader(b200q_file_reader_fn fn, void* ctx);   /* process-wide; fn = NULL restores local files */
+/* ---- Scalar subqueries: the bloom filter of BloomFilterMightContain -------------------------------------------------------
+ * Reference: SparkScalarSubqueryWrapperExpr::evaluate (datafusion-ext-exprs/src/spark_scalar_subquery_wrapper.rs:109-129), which
+ * runs the subquery on the JVM through the wrapper's `serialized` bytes.  Spark's runtime bloom filters place such a wrapper as the
+ * filter argument of BloomFilterMightContain; the library evaluates nothing on the JVM, so it asks the host once per
+ * BloomFilterMightContain at b200q_op_create (b200q_plan_explain never asks).  `fn` gets the wrapper's serialized bytes and
+ * returns 0 after calling `put(sink, value, len)` once with the Binary value (the library copies it before `put` returns), or
+ * returns 0 without calling `put` when the value is NULL (the filter then matches no row).  Any other return value fails the
+ * create with B200Q_ERR_EXECUTION.  Without a resolver such plans are B200Q_ERR_UNSUPPORTED. */
+typedef void (*b200q_bytes_sink_fn)(void* sink, const uint8_t* value, size_t len);
+typedef int32_t (*b200q_scalar_subquery_fn)(void* ctx, const uint8_t* serialized, size_t len, b200q_bytes_sink_fn put, void* sink);
+b200q_status b200q_set_scalar_subquery_resolver(b200q_scalar_subquery_fn fn, void* ctx);   /* process-wide; fn = NULL removes it */
+
 /* Host-only helpers of the scan (no GPU needed; debugging and the CPU test-suite): render a Thrift-encoded FileMetaData footer
  * (columns with their Arrow mapping, row groups, codecs, statistics) as text; raw Snappy decompression of one page body. */
 b200q_status b200q_parquet_explain(const uint8_t* footer, size_t n, char* buf, size_t cap, size_t* needed);

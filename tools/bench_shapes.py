@@ -129,6 +129,62 @@ vbits = torch.full(((rows + 7) // 8,), 0xFF, dtype=torch.uint8, device=dev); vbi
 s2t = T.Schema([T.Field("f", T.int64, False), T.Field("k1", T.int32, False), T.Field("k2", T.int64, False), T.Field("v", T.int64, True)])
 run("M2 int32 key, nullable v", m2s(s2t, 200, 399).plan_bytes(), [f, k1_32, k2, v], 28.125, native.default_conf(agg_initial_groups=1 << 20), valid=[None, None, None, vbits])
 del k1_32, vbits
+# BF1: a Spark runtime bloom filter on the fact side: Filter(might_contain(XxHash64(k1))) -> SUM(v) GROUP BY k2 over an 8 MiB filter
+# (2^26 bits, k = 6) holding 10 % of the k1 domain, so about 10 % of the rows pass  (24 B/row: k1, k2, v).  Next to it: the same
+# aggregate without the conjunct (fast kernels), and with a plain `k1 < lit` conjunct of the same selectivity under
+# force_generic_kernels: the difference to the latter is the probe, to the former the cost of leaving the fast kernels too.
+# BF2: the creation side, BLOOM_FILTER(XxHash64(k1), 10^6 items, 2^26 bits) over 2^26 rows, Partial + Final fused in one op (8 B/row).
+# Whole-op wall time (push_device .. finish .. pull .. sync, op create outside) next to the hot-kernel time; the card and its power
+# limit are read in the same process
+def run_wall(name, plan_bytes, cols, n, alg_bytes_per_row, conf=None, reps=3):
+    import time
+    spec = [(c.data_ptr(), 0, n) for c in cols]
+    best = None
+    for _ in range(REPS or reps):
+        with native.NativeOp(plan_bytes, conf or native.default_conf(), 0) as op:
+            torch.cuda.synchronize(); t0 = time.perf_counter()
+            op.push_device(native.DeviceBatch(spec, n, 0, keepalive=list(cols)))
+            op.finish()
+            while True:
+                o = op.pull_device()
+                if o is None: break
+                native.release_device_array(o)
+            op.sync(); wall = time.perf_counter() - t0
+            m = op.metrics()
+        if best is None or wall < best[0]: best = (wall, m)
+    wall, m = best
+    print(json.dumps({"shape": name, "rows": n, "wall_ms": wall * 1e3, "rows_per_s": n / wall, "alg_GBps_wall": alg_bytes_per_row * n / wall / 1e9,
+                      "frac_of_hbm_peak_wall": alg_bytes_per_row * n / wall / 1e9 / peak, "hot_kernel_ms": m["hot_kernel_ns"] / 1e6,
+                      "fast_path_launches": m["fast_path_launches"], "launches": m["gpu_kernel_launches"], "gpu": card}), flush=True)
+
+if not ONLY or any(t in "BF1 BF2" for t in ONLY.split(",")):
+    import subprocess
+    from oracle import bloom_oracle as BO
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True).stdout.strip()
+    if not ONLY or "BF1" in ONLY:
+        bf = BO.SparkBloomFilter(6, BO.SparkBitArray.with_num_bits(1 << 26))
+        for key in range((1 << 17) // 10):
+            bf.put_long(BO.xxhash64(key.to_bytes(8, "little", signed=True), 42))
+        bf_lit = E.Literal(bf.write_to(), T.binary)
+        bf_agg = lambda pred: PL.AggExec(PL.HashAgg, [E.GroupingExpr("k2", E.Column("k2"))],
+                                         [E.AggExpr("s", E.PARTIAL, PL.create_agg(E.AGG_SUM, [E.Column("v")], s2, T.int64))], True,
+                                         PL.FilterExec([pred], PL.MemoryExec(s2)) if pred is not None else PL.MemoryExec(s2))
+        run_wall("BF1 might_contain(XxHash64(k1)) -> SUM(v) GROUP BY k2, 8 MiB filter, s~0.1",
+                 bf_agg(E.BloomFilterMightContain(bf_lit, E.XxHash64(E.Column("k1")), "bf1")).plan_bytes(), [f, k1, k2, v], rows, 24.0)
+        run_wall("BF1 same aggregate without the bloom conjunct", bf_agg(None).plan_bytes(), [f, k1, k2, v], rows, 24.0)
+        run_wall("BF1 same aggregate, k1 < 13107 under force_generic_kernels",
+                 bf_agg(E.BinaryExpr(E.Column("k1"), "Lt", E.Literal((1 << 17) // 10, T.int64))).plan_bytes(), [f, k1, k2, v], rows, 24.0,
+                 native.default_conf(force_generic_kernels=1))
+        del bf, bf_lit
+    if not ONLY or "BF2" in ONLY:
+        n2 = min(rows, 1 << 26)
+        sk = T.Schema([T.Field("k1", T.int64, False)])
+        mk_bf = lambda mode, ch, sch: [E.AggExpr("bf", mode, PL.create_agg(E.AGG_BLOOM_FILTER, [ch, E.Literal(10**6, T.int64), E.Literal(1 << 26, T.int64)], sch, T.binary))]
+        bf_p = PL.AggExec(PL.HashAgg, [], mk_bf(E.PARTIAL, E.XxHash64(E.Column("k1")), sk), False, PL.MemoryExec(sk))
+        bf_f = PL.AggExec(PL.HashAgg, [], mk_bf(E.FINAL, E.placeholder(T.binary), bf_p.schema()), False, bf_p)
+        k1_2 = k1[:n2].contiguous()
+        run_wall("BF2 BLOOM_FILTER(XxHash64(k1)) build, 2^26 bits, Partial + Final fused", bf_f.plan_bytes(), [k1_2], n2, 8.0)
+        del k1_2
 # M3: ShuffleWriterExec 200-way hash partition + batch_serde encode (BASELINE configs[3] map side): 32 B/row read + 32 B/row of byte planes written
 m3 = PL.ShuffleWriterExec(PL.MemoryExec(s2), ("hash", [E.Column("k1")], 200), "", "")
 run("M3 shuffle write 200-way (4 int64 columns, hash on k1)", m3.plan_bytes(), [f, k1, k2, v], 64.0, native.default_conf(shuffle_output_on_device=1), reps=2)
