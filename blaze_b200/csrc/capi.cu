@@ -99,6 +99,7 @@ struct b200q_op {
   StagingSet staging[2]; int cur_stage_set = 0; bool staging_ready = false;
   cudaEvent_t ev_a = nullptr, ev_b = nullptr;
   std::shared_ptr<StreamRef> stream_ref;
+  const PlanNode* leaf = nullptr;   // the plan's leaf (owned by `plan`)
   std::unique_ptr<IpcSource> ipc;   // the op's source when its leaf is an IpcReaderExecNode (input through b200q_op_push_ipc only)
   bool taken = false;               // its output became the right side of a sort-merge join (b200q_op_attach_right)
 };
@@ -165,6 +166,12 @@ static bool fusable_partial_final(const PlanNode& p, const PlanNode& f) {
   return true;
 }
 
+static std::vector<ExprP> substitute_all(const std::vector<ExprP>& exprs, const std::vector<ExprP>& cols) {
+  std::vector<ExprP> v;
+  for (auto& e : exprs) v.push_back(substitute(e, cols));
+  return v;
+}
+
 static void build_pipeline(b200q_op* op) {
   std::vector<PlanNode*> chain;
   for (PlanNode* n = op->plan.get(); n; n = n->input.get()) chain.push_back(n);
@@ -173,50 +180,54 @@ static void build_pipeline(b200q_op* op) {
   if (chain[0]->leaf_kind == "ParquetScan")
     for (auto& f : chain[0]->schema.fields)
       if (f.type.is_varlen()) throw PlanError(B200Q_ERR_UNSUPPORTED, "ParquetScanExec: column " + f.name + " is " + f.type.str() + "; BYTE_ARRAY decode is not on the GPU path");
+  op->leaf = chain[0];
   op->in_schema = chain[0]->schema;
   SchemaDef stage_in = chain[0]->schema;
   std::vector<ExprP> cur_cols = identity_cols(stage_in), filters;
-  const PlanNode* last = chain[0];
   bool pending_tail = chain.size() == 1;
-  // the aggregate chain[i] over the columns of each set (one set: `cur_cols`); on return chain[i] is the last node the stage consumed
-  auto push_agg = [&](size_t& i, const std::vector<std::vector<ExprP>>& set_cols) {
-    PlanNode* n = chain[i];
-    std::vector<AggSetExprs> sets;
-    for (auto& cols : set_cols) {
-      AggSetExprs sx;
-      for (auto& g : n->group_exprs) sx.group_exprs.push_back(substitute(g, cols));
-      for (auto& a : n->aggs) { std::vector<ExprP> v; if (a.mode == MODE_PARTIAL) for (auto& e : a.args) v.push_back(substitute(e, cols)); sx.agg_args.push_back(v); }
-      sets.push_back(std::move(sx));
-    }
-    // AggExec(Final) directly above AggExec(Partial) in the same op (Spark plans this when the child is already partitioned on the grouping keys):
-    // the Partial stage's table holds one entry per group, so a Final stage would only re-insert unique keys into a second table.  One stage
-    // accumulates from the raw inputs and emits the Final columns (AVG division, result types) straight from its table.
-    PlanNode fused;
-    const PlanNode* agg_node = n;
-    last = n;
-    if (i + 1 < chain.size() && fusable_partial_final(*n, *chain[i + 1])) {
-      fused = *n; fused.need_final_merge = true; fused.schema = chain[i + 1]->schema;
-      agg_node = &fused; last = chain[i + 1]; i++;
-    }
-    if (sets.size() > 1) op->stages.push_back(make_agg_stage(op->cx, stage_in, filters, *agg_node, sets[0].group_exprs, sets[0].agg_args, sets));
-    else op->stages.push_back(make_agg_stage(op->cx, stage_in, filters, *agg_node, sets[0].group_exprs, sets[0].agg_args));
+  // the next stage reads the output of the last one.  `filters` is non-empty only while `pending_tail` is set (a FilterExec and a
+  // window group limit both set it), so a stage that does not consume a pending Filter / Project chain finds nothing to reset
+  auto add = [&](std::unique_ptr<Stage> st) {
+    op->stages.push_back(std::move(st));
     stage_in = op->stages.back()->out_schema;
     cur_cols = identity_cols(stage_in); filters.clear(); pending_tail = false;
   };
+  // the pending Filter / Project chain as its own fused stage, writing `outs` as `schema`
+  auto flush = [&](const std::vector<ExprP>& outs, const SchemaDef& schema) { add(make_filter_project_stage(op->cx, stage_in, filters, outs, schema)); };
+  // AggExec(Final) directly above AggExec(Partial) in the same op (Spark plans this when the child is already partitioned on the grouping keys):
+  // the Partial stage's table holds one entry per group, so a Final stage would only re-insert unique keys into a second table.  One stage
+  // accumulates from the raw inputs and emits the Final columns (AVG division, result types) straight from its table.  Returns the node
+  // the stage runs: chain[i], or chain[i] fused with the Final above it, and then i is the Final's
+  auto fuse_final = [&](size_t& i) {
+    PlanNode node = *chain[i];
+    if (i + 1 < chain.size() && fusable_partial_final(node, *chain[i + 1])) {
+      node.need_final_merge = true; node.schema = chain[i + 1]->schema;
+      i++;
+    }
+    return node;
+  };
+  // the aggregate chain[i] over the columns of each set (one set: `cur_cols`); on return chain[i] is the last node the stage consumed
+  auto push_agg = [&](size_t& i, const std::vector<std::vector<ExprP>>& set_cols) {
+    const PlanNode* n = chain[i];
+    std::vector<AggSetExprs> sets;
+    for (auto& cols : set_cols) {
+      AggSetExprs sx;
+      sx.group_exprs = substitute_all(n->group_exprs, cols);
+      for (auto& a : n->aggs) sx.agg_args.push_back(a.mode == MODE_PARTIAL ? substitute_all(a.args, cols) : std::vector<ExprP>());
+      sets.push_back(std::move(sx));
+    }
+    const PlanNode node = fuse_final(i);
+    if (sets.size() > 1) add(make_agg_stage(op->cx, stage_in, filters, node, sets[0].group_exprs, sets[0].agg_args, sets));
+    else add(make_agg_stage(op->cx, stage_in, filters, node, sets[0].group_exprs, sets[0].agg_args));
+  };
   for (size_t i = 1; i < chain.size(); i++) {
     PlanNode* n = chain[i];
-    last = n;
-    if (n->kind == N_FILTER) { for (auto& p : n->predicates) filters.push_back(substitute(p, cur_cols)); pending_tail = true; }
-    else if (n->kind == N_PROJECT) { std::vector<ExprP> nc; for (auto& e : n->proj_exprs) nc.push_back(substitute(e, cur_cols)); cur_cols = nc; pending_tail = true; }
+    if (n->kind == N_FILTER) { for (auto& p : substitute_all(n->predicates, cur_cols)) filters.push_back(p); pending_tail = true; }
+    else if (n->kind == N_PROJECT) { cur_cols = substitute_all(n->proj_exprs, cur_cols); pending_tail = true; }
     else if (n->kind == N_AGG && !n->aggs.empty() && n->aggs[0].fn == AGG_BLOOM_FILTER) {
       // BLOOM_FILTER (decode admits it only without grouping keys and next to other BLOOM_FILTERs): a stage of its own.  Computed
       // values (the usual XxHash64(col)) and any filter below come from a FilterProjectStage, as trailing columns
-      PlanNode fused;
-      const PlanNode* node = n;
-      if (i + 1 < chain.size() && fusable_partial_final(*n, *chain[i + 1])) {
-        fused = *n; fused.need_final_merge = true; fused.schema = chain[i + 1]->schema;
-        node = &fused; last = chain[i + 1]; i++;
-      }
+      const PlanNode node = fuse_final(i);
       std::vector<int> vcols;
       SchemaDef bin = stage_in;
       if (n->need_partial_update) {
@@ -232,38 +243,32 @@ static void build_pipeline(b200q_op* op) {
         else {
           bin = SchemaDef();
           for (size_t k = 0; k < vals.size(); k++) { bin.fields.push_back(FieldDef{"#bloom_arg" + std::to_string(k), vals[k]->type, vals[k]->nullable}); vcols.push_back((int)k); }
-          op->stages.push_back(make_filter_project_stage(op->cx, stage_in, filters, vals, bin));
+          flush(vals, bin);
         }
       } else if (!filters.empty() || !is_identity(cur_cols, stage_in)) {
         throw PlanError(B200Q_ERR_UNSUPPORTED, "Filter / Projection fused below a merge-mode BLOOM_FILTER aggregate");
       }
-      op->stages.push_back(make_bloom_agg_stage(op->cx, bin, *node, vcols));
-      stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in); filters.clear(); pending_tail = false;
+      add(make_bloom_agg_stage(op->cx, bin, node, vcols));
     } else if (n->kind == N_AGG) {
       if (n->need_partial_merge && !is_identity(cur_cols, stage_in)) throw PlanError(B200Q_ERR_UNSUPPORTED, "Projection fused below a merge-mode aggregate");
       push_agg(i, {cur_cols});
     } else if (n->kind == N_EXPAND) {
       std::vector<std::vector<ExprP>> sets;
-      for (auto& proj : n->expand_projections) { std::vector<ExprP> v; for (auto& e : proj) v.push_back(substitute(e, cur_cols)); sets.push_back(v); }
+      for (auto& proj : n->expand_projections) sets.push_back(substitute_all(proj, cur_cols));
       if (sets.size() == 1) { cur_cols = sets[0]; pending_tail = true; continue; }       // one projection: a ProjectExec
       // Expand -> [Project]* -> AggExec(Partial): the sets are fused into the aggregate (each input row is read once and inserted once per
       // set; filters below the Expand are shared by all sets).  Anything else above the Expand sees it materialised.
       std::vector<std::vector<ExprP>> composed = sets;
       size_t j = i + 1;
       for (; j < chain.size() && chain[j]->kind == N_PROJECT; j++)
-        for (auto& cols : composed) { std::vector<ExprP> nc; for (auto& e : chain[j]->proj_exprs) nc.push_back(substitute(e, cols)); cols = nc; }
+        for (auto& cols : composed) cols = substitute_all(chain[j]->proj_exprs, cols);
       bool fuse = sets.size() > 1 && j < chain.size() && chain[j]->kind == N_AGG && !chain[j]->need_partial_merge;
       if (fuse) for (auto& a : chain[j]->aggs) fuse = fuse && a.mode == MODE_PARTIAL && a.fn != AGG_BLOOM_FILTER;
       if (fuse) { i = j; push_agg(i, composed); continue; }
-      op->stages.push_back(make_expand_stage(op->cx, stage_in, filters, sets, n->schema));
-      stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in); filters.clear(); pending_tail = false;
+      add(make_expand_stage(op->cx, stage_in, filters, sets, n->schema));
     } else if (n->kind == N_SORT) {
-      if (pending_tail) {
-        op->stages.push_back(make_filter_project_stage(op->cx, stage_in, filters, cur_cols, n->input->schema));
-        stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in); filters.clear(); pending_tail = false;
-      }
-      op->stages.push_back(make_sort_stage(op->cx, stage_in, *n));
-      stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in);
+      if (pending_tail) flush(cur_cols, n->input->schema);
+      add(make_sort_stage(op->cx, stage_in, *n));
     } else if (n->kind == N_WINDOW) {
       // a WindowExec without a limit directly on one with a limit runs as ONE window: the parent's expressions, the child's
       // limit, output_window_cols = true, over the child's input (window_exec.rs:166-185)
@@ -276,7 +281,7 @@ static void build_pipeline(b200q_op* op) {
         combined = *chain[i + 1]; combined.window_has_limit = true; combined.window_limit = n->window_limit; combined.output_window_cols = true;
         if (combined.window_exprs.size() != 1) throw PlanError(B200Q_ERR_INVALID_PLAN, "WindowExec: a group limit needs exactly one window expression, got " + std::to_string(combined.window_exprs.size()));
         if (!combined.window_exprs[0].is_rank) throw PlanError(B200Q_ERR_UNSUPPORTED, "WindowExec: a group limit over an aggregate window column is not on the GPU path (rank-like functions are)");
-        w = &combined; i++; last = chain[i];
+        w = &combined; i++;
       }
       // keys and arguments that are not input columns are computed by a FilterProjectStage below, as trailing columns
       const size_t n_fwd = w->input->schema.fields.size();
@@ -295,12 +300,10 @@ static void build_pipeline(b200q_op* op) {
       for (auto& we : w->window_exprs) { std::vector<int> v; if (!we.is_rank) for (auto& a : we.agg.args) v.push_back(col_of(a)); wc.agg_args.push_back(v); }
       if (pending_tail || !extra.empty()) {
         std::vector<ExprP> outs = cur_cols;
-        for (auto& e : extra) outs.push_back(substitute(e, cur_cols));
-        op->stages.push_back(make_filter_project_stage(op->cx, stage_in, filters, outs, win_in));
-        filters.clear(); pending_tail = false;
+        for (auto& e : substitute_all(extra, cur_cols)) outs.push_back(e);
+        flush(outs, win_in);
       }
-      op->stages.push_back(make_window_stage(op->cx, win_in, *w, wc));
-      stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in);
+      add(make_window_stage(op->cx, win_in, *w, wc));
       if (w->window_has_limit) {
         // WindowGroupLimit: keep the rows whose window column is <= (int32)k (window_exec.rs:227-235); the window column is dropped
         // unless output_window_cols.  A pending filter, fused into whatever runs next.
@@ -312,38 +315,23 @@ static void build_pipeline(b200q_op* op) {
         if (!w->output_window_cols) cur_cols.resize(n_fwd);
         pending_tail = true;
       }
-    } else if (n->kind == N_JOIN_BUILD || n->kind == N_JOIN) {
-      if (pending_tail) {                               // Filter / Project chain below the join side: its own fused stage
-        op->stages.push_back(make_filter_project_stage(op->cx, stage_in, filters, cur_cols, n->input->schema));
-        stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in); filters.clear(); pending_tail = false;
-      }
-      if (n->kind == N_JOIN_BUILD) {
-        if (i + 1 != chain.size()) throw PlanError(B200Q_ERR_UNSUPPORTED, "BroadcastJoinBuildHashMapExec below another operator: build the map side with its own op and attach it (b200q_op_attach_build)");
-        op->stages.push_back(make_join_build_stage(op->cx, stage_in, *n));
-      } else {
-        op->stages.push_back(make_join_probe_stage(op->cx, stage_in, *n));
-        stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in);
-      }
+    } else if (n->kind == N_JOIN_BUILD) {
+      if (pending_tail) flush(cur_cols, n->input->schema);      // Filter / Project chain below the join side: its own fused stage
+      if (i + 1 != chain.size()) throw PlanError(B200Q_ERR_UNSUPPORTED, "BroadcastJoinBuildHashMapExec below another operator: build the map side with its own op and attach it (b200q_op_attach_build)");
+      add(make_join_build_stage(op->cx, stage_in, *n));
+    } else if (n->kind == N_JOIN) {
+      if (pending_tail) flush(cur_cols, n->input->schema);
+      add(make_join_probe_stage(op->cx, stage_in, *n));
     } else if (n->kind == N_SMJ) {
-      if (pending_tail) {                               // Filter / Project chain below the left side: its own fused stage
-        op->stages.push_back(make_filter_project_stage(op->cx, stage_in, filters, cur_cols, n->input->schema));
-        stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in); filters.clear(); pending_tail = false;
-      }
-      op->stages.push_back(make_smj_stage(op->cx, stage_in, *n));
-      stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in);
+      if (pending_tail) flush(cur_cols, n->input->schema);      // Filter / Project chain below the left side
+      add(make_smj_stage(op->cx, stage_in, *n));
     } else if (n->kind == N_SHUFFLE_WRITER) {
       if (i + 1 != chain.size()) throw PlanError(B200Q_ERR_UNSUPPORTED, "ShuffleWriterExec below another operator");
-      if (pending_tail) {                               // Filter / Project chain below the writer: its own fused stage
-        op->stages.push_back(make_filter_project_stage(op->cx, stage_in, filters, cur_cols, n->input->schema));
-        stage_in = op->stages.back()->out_schema; cur_cols = identity_cols(stage_in); filters.clear(); pending_tail = false;
-      }
-      op->stages.push_back(make_shuffle_write_stage(op->cx, stage_in, *n));
+      if (pending_tail) flush(cur_cols, n->input->schema);
+      add(make_shuffle_write_stage(op->cx, stage_in, *n));
     } else throw PlanError(B200Q_ERR_INVALID_PLAN, "leaf in the middle of the plan");
   }
-  if (pending_tail) {
-    SchemaDef out = last->schema;
-    op->stages.push_back(make_filter_project_stage(op->cx, stage_in, filters, cur_cols, out));
-  }
+  if (pending_tail) flush(cur_cols, chain.back()->schema);
   op->out_schema = op->stages.back()->out_schema;
 }
 
@@ -396,50 +384,80 @@ static void poll_pending(b200q_op* op, bool wait) {
   }
 }
 
+// the state checks b200q_op_push and b200q_op_push_device start with
+static void check_push_state(b200q_op* op) {
+  if (op->finished) throw ExecError(B200Q_ERR_STATE, "push after finish");
+  if (op->ipc) throw ExecError(B200Q_ERR_STATE, "an op whose leaf is an IpcReaderExecNode takes its input through b200q_op_push_ipc");
+}
+// their common start once the batch is known to be there: the sort-merge join's right side, the device, the batch's columns, and
+// the releases whose copies have drained
+static void begin_push(b200q_op* op, const ArrowArray* batch) {
+  require_right_side(op);
+  B200Q_CUDA(cudaSetDevice(op->cx.device));
+  validate_host_batch(op, batch);
+  poll_pending(op, false);
+}
+
+// the leaf's columns, typed, for `rows` rows; each import fills the columns the first stage reads
+static DevBatch input_batch(b200q_op* op, int64_t rows) {
+  DevBatch db; db.num_rows = rows; db.cols.resize(op->in_schema.fields.size());
+  for (size_t i = 0; i < db.cols.size(); i++) db.cols[i].type = op->in_schema.fields[i].type;
+  return db;
+}
+
+// uploads rows [a0, a0 + cnt) of one host column into `dc`; a0 is a multiple of 8, so the bitmaps (`validity`, null when the column
+// has no nulls, and Boolean `values`) start at a byte.  Varlen offsets are rebased to 0 on the device, and `data` holds the `data_len`
+// bytes from the one offsets[a0] names
+static void upload_column(OpContext& cx, DevColumn& dc, int64_t a0, int64_t cnt, const uint8_t* validity, const void* values,
+                          const int32_t* offsets, const uint8_t* data, size_t data_len) {
+  if (validity) {
+    const size_t nb = (size_t)((cnt + 7) / 8);
+    dc.validity = DevMem::alloc(nb + 4, cx.stream);
+    B200Q_CUDA(cudaMemcpyAsync(dc.validity->ptr, validity + a0 / 8, nb, cudaMemcpyHostToDevice, cx.stream)); cx.m.h2d_bytes += (int64_t)nb;
+  }
+  if (dc.type.is_varlen()) {
+    const int32_t* offs = offsets + a0;
+    dc.offsets = DevMem::alloc((size_t)(cnt + 1) * 4, cx.stream);
+    // the device offsets start at 0, so every imported column indexes its own allocation (columns may then be shared with the
+    // output and exported as they are)
+    if (offs[0] == 0) B200Q_CUDA(cudaMemcpyAsync(dc.offsets->ptr, offs, (size_t)(cnt + 1) * 4, cudaMemcpyHostToDevice, cx.stream));
+    else {
+      std::vector<int32_t> rebased(offs, offs + cnt + 1);
+      for (auto& o : rebased) o -= offs[0];
+      // a pageable source: the call returns once `rebased` has been staged, so it may go out of scope
+      B200Q_CUDA(cudaMemcpyAsync(dc.offsets->ptr, rebased.data(), (size_t)(cnt + 1) * 4, cudaMemcpyHostToDevice, cx.stream));
+    }
+    dc.values = DevMem::alloc(data_len, cx.stream);
+    if (data_len) B200Q_CUDA(cudaMemcpyAsync(dc.values->ptr, data, data_len, cudaMemcpyHostToDevice, cx.stream));
+    cx.m.h2d_bytes += (int64_t)(cnt + 1) * 4 + (int64_t)data_len;
+  } else if (dc.type.id == T_BOOL) {
+    const size_t nb = (size_t)((cnt + 7) / 8);
+    dc.values = DevMem::alloc(nb + 4, cx.stream);
+    B200Q_CUDA(cudaMemcpyAsync(dc.values->ptr, (const uint8_t*)values + a0 / 8, nb, cudaMemcpyHostToDevice, cx.stream)); cx.m.h2d_bytes += (int64_t)nb;
+  } else if (dc.type.id != T_NULL) {
+    const size_t w = (size_t)dc.type.byte_width(), nb = (size_t)cnt * w;
+    dc.values = DevMem::alloc(nb, cx.stream);
+    B200Q_CUDA(cudaMemcpyAsync(dc.values->ptr, (const uint8_t*)values + (size_t)a0 * w, nb, cudaMemcpyHostToDevice, cx.stream)); cx.m.h2d_bytes += (int64_t)nb;
+  }
+}
+
 // direct path: each used column is copied straight from the caller's buffers
 static DevBatch import_direct(b200q_op* op, const ArrowArray* batch, const std::vector<int>& used) {
-  OpContext& cx = op->cx;
-  DevBatch db; db.num_rows = batch->length; db.cols.resize(op->in_schema.fields.size());
-  for (size_t i = 0; i < db.cols.size(); i++) db.cols[i].type = op->in_schema.fields[i].type;
+  DevBatch db = input_batch(op, batch->length);
   for (int ci : used) {
     const ArrowArray* c = batch->children[ci];
     DevColumn& dc = db.cols[ci];
     const int64_t off = c->offset + batch->offset, len = batch->length;
     const int64_t a0 = off & ~7LL;                    // align down to a byte of the bitmaps
     dc.offset = off - a0;
-    const int64_t cnt = dc.offset + len;
-    const uint8_t* validity = c->n_buffers > 0 ? (const uint8_t*)c->buffers[0] : nullptr;
-    if (validity && c->null_count != 0) {
-      const size_t nb = (size_t)((cnt + 7) / 8);
-      dc.validity = DevMem::alloc(nb + 4, cx.stream);
-      B200Q_CUDA(cudaMemcpyAsync(dc.validity->ptr, validity + a0 / 8, nb, cudaMemcpyHostToDevice, cx.stream)); cx.m.h2d_bytes += (int64_t)nb;
-    }
-    if (dc.type.is_varlen()) {
+    const uint8_t* validity = c->n_buffers > 0 && c->null_count != 0 ? (const uint8_t*)c->buffers[0] : nullptr;
+    const int32_t* offs = nullptr; const uint8_t* data = nullptr; size_t data_len = 0;
+    if (dc.type.is_varlen()) {                        // only the bytes the rows reference are copied
       if (c->n_buffers < 3) throw ExecError(B200Q_ERR_INVALID_ARG, dc.type.str() + " column needs 3 buffers");
-      const int32_t* offs = (const int32_t*)c->buffers[1]; const uint8_t* data = (const uint8_t*)c->buffers[2];
-      const int32_t first = offs[a0], end = offs[off + len];
-      dc.offsets = DevMem::alloc((size_t)(cnt + 1) * 4, cx.stream);
-      // only [first, end) of the data is copied: the device offsets are rebased to start at 0, so every imported column indexes its
-      // own allocation (columns may then be shared with the output and exported as they are)
-      if (first == 0) B200Q_CUDA(cudaMemcpyAsync(dc.offsets->ptr, offs + a0, (size_t)(cnt + 1) * 4, cudaMemcpyHostToDevice, cx.stream));
-      else {
-        std::vector<int32_t> rebased(offs + a0, offs + a0 + cnt + 1);
-        for (auto& o : rebased) o -= first;
-        // a pageable source: the call returns once `rebased` has been staged, so it may go out of scope
-        B200Q_CUDA(cudaMemcpyAsync(dc.offsets->ptr, rebased.data(), (size_t)(cnt + 1) * 4, cudaMemcpyHostToDevice, cx.stream));
-      }
-      dc.values = DevMem::alloc((size_t)(end - first), cx.stream);
-      if (end > first) B200Q_CUDA(cudaMemcpyAsync(dc.values->ptr, data + first, (size_t)(end - first), cudaMemcpyHostToDevice, cx.stream));
-      cx.m.h2d_bytes += (int64_t)(cnt + 1) * 4 + (end - first);
-    } else if (dc.type.id == T_BOOL) {
-      const size_t nb = (size_t)((cnt + 7) / 8);
-      dc.values = DevMem::alloc(nb + 4, cx.stream);
-      B200Q_CUDA(cudaMemcpyAsync(dc.values->ptr, (const uint8_t*)c->buffers[1] + a0 / 8, nb, cudaMemcpyHostToDevice, cx.stream)); cx.m.h2d_bytes += (int64_t)nb;
-    } else if (dc.type.id != T_NULL) {
-      const size_t w = (size_t)dc.type.byte_width();
-      dc.values = DevMem::alloc((size_t)cnt * w, cx.stream);
-      B200Q_CUDA(cudaMemcpyAsync(dc.values->ptr, (const uint8_t*)c->buffers[1] + (size_t)a0 * w, (size_t)cnt * w, cudaMemcpyHostToDevice, cx.stream)); cx.m.h2d_bytes += (int64_t)(cnt * w);
+      offs = (const int32_t*)c->buffers[1];
+      data = (const uint8_t*)c->buffers[2] + offs[a0]; data_len = (size_t)(offs[off + len] - offs[a0]);
     }
+    upload_column(op->cx, dc, a0, dc.offset + len, validity, dc.type.id == T_NULL ? nullptr : c->buffers[1], offs, data, data_len);
   }
   return db;
 }
@@ -477,19 +495,10 @@ static void staging_flush(b200q_op* op) {
   StagingSet& st = op->staging[op->cur_stage_set];
   if (st.rows == 0) return;
   OpContext& cx = op->cx;
-  const std::vector<int>& used = op->stages[0]->used_input_cols;
-  DevBatch db; db.num_rows = st.rows; db.cols.resize(op->in_schema.fields.size());
-  for (size_t i = 0; i < db.cols.size(); i++) db.cols[i].type = op->in_schema.fields[i].type;
-  for (int ci : used) {
-    StagingSet::Col& c = st.cols[ci]; DevColumn& dc = db.cols[ci];
-    const int64_t n = st.rows;
-    if (c.validity && c.any_null) { const size_t nb = (size_t)(n + 7) / 8; dc.validity = DevMem::alloc(nb + 4, cx.stream); B200Q_CUDA(cudaMemcpyAsync(dc.validity->ptr, c.validity, nb, cudaMemcpyHostToDevice, cx.stream)); cx.m.h2d_bytes += (int64_t)nb; }
-    if (dc.type.is_varlen()) {
-      dc.offsets = DevMem::alloc((size_t)(n + 1) * 4, cx.stream); B200Q_CUDA(cudaMemcpyAsync(dc.offsets->ptr, c.offsets, (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, cx.stream));
-      dc.values = DevMem::alloc(c.data_len, cx.stream); if (c.data_len) B200Q_CUDA(cudaMemcpyAsync(dc.values->ptr, c.data, c.data_len, cudaMemcpyHostToDevice, cx.stream));
-      cx.m.h2d_bytes += (int64_t)(n + 1) * 4 + (int64_t)c.data_len;
-    } else if (dc.type.id == T_BOOL) { const size_t nb = (size_t)(n + 7) / 8; dc.values = DevMem::alloc(nb + 4, cx.stream); B200Q_CUDA(cudaMemcpyAsync(dc.values->ptr, c.values, nb, cudaMemcpyHostToDevice, cx.stream)); cx.m.h2d_bytes += (int64_t)nb; }
-    else if (dc.type.id != T_NULL) { const size_t nb = (size_t)n * dc.type.byte_width(); dc.values = DevMem::alloc(nb, cx.stream); B200Q_CUDA(cudaMemcpyAsync(dc.values->ptr, c.values, nb, cudaMemcpyHostToDevice, cx.stream)); cx.m.h2d_bytes += (int64_t)nb; }
+  DevBatch db = input_batch(op, st.rows);
+  for (int ci : op->stages[0]->used_input_cols) {
+    StagingSet::Col& c = st.cols[ci];
+    upload_column(cx, db.cols[ci], 0, st.rows, c.any_null ? c.validity : nullptr, c.values, c.offsets, c.data, c.data_len);
   }
   B200Q_CUDA(cudaEventRecord(st.ev, cx.stream)); st.in_flight = true;
   // switch to the other set; wait until its previous H2D has drained before it is overwritten
@@ -536,14 +545,18 @@ static void staging_append(b200q_op* op, const ArrowArray* batch) {
 }
 
 // ---- stage driver ----------------------------------------------------------------------------------------
+// the outputs of stage i go to stage i + 1, or out of the op
+static void route_outputs(b200q_op* op, size_t i, std::vector<DevBatch>& outs) {
+  for (auto& o : outs) {
+    if (i + 1 < op->stages.size()) run_stages(op, o, i + 1);
+    else { op->cx.m.output_rows += o.num_rows; op->out_queue.push_back(std::move(o)); }
+  }
+}
 static void run_stages(b200q_op* op, DevBatch& b, size_t from) {
   std::vector<DevBatch> outs;
   op->cx.cur_stage = (int)from;
   op->stages[from]->push(op->cx, b, outs);
-  for (auto& o : outs) {
-    if (from + 1 < op->stages.size()) run_stages(op, o, from + 1);
-    else { op->cx.m.output_rows += o.num_rows; op->out_queue.push_back(std::move(o)); }
-  }
+  route_outputs(op, from, outs);
 }
 
 // ---- device -> host export ---------------------------------------------------------------------------------
@@ -708,9 +721,7 @@ b200q_status b200q_op_create(const uint8_t* plan, size_t plan_len, int32_t plan_
     op->cx.stream = op->stream_ref->s;
     B200Q_CUDA(cudaEventCreate(&op->cx.ev0)); B200Q_CUDA(cudaEventCreate(&op->cx.ev1));
     build_pipeline(op);
-    const PlanNode* leaf = op->plan.get();
-    while (leaf->input) leaf = leaf->input.get();
-    if (leaf->leaf_kind == "IpcReader") op->ipc = make_ipc_source(op->cx, op->in_schema, op->stages[0]->used_input_cols);
+    if (op->leaf->leaf_kind == "IpcReader") op->ipc = make_ipc_source(op->cx, op->in_schema, op->stages[0]->used_input_cols);
     if (input_schema) {
       if (input_schema->n_children != (int64_t)op->in_schema.fields.size()) throw PlanError(B200Q_ERR_INVALID_ARG, "input_schema does not match the plan leaf: column count");
       for (int64_t i = 0; i < input_schema->n_children; i++)
@@ -735,12 +746,8 @@ b200q_status b200q_op_output_schema(b200q_op* op, struct ArrowSchema* out) {
 b200q_status b200q_op_push(b200q_op* op, struct ArrowArray* batch) {
   if (!op) return fail(B200Q_ERR_INVALID_ARG, "op is null");
   b200q_status st = guarded(op, [&] {
-    if (op->finished) throw ExecError(B200Q_ERR_STATE, "push after finish");
-    if (op->ipc) throw ExecError(B200Q_ERR_STATE, "an op whose leaf is an IpcReaderExecNode takes its input through b200q_op_push_ipc");
-    require_right_side(op);
-    B200Q_CUDA(cudaSetDevice(op->cx.device));
-    validate_host_batch(op, batch);
-    poll_pending(op, false);
+    check_push_state(op);
+    begin_push(op, batch);
     op->cx.m.input_rows += batch->length; op->cx.m.input_batches++;
     if (batch->length == 0) return;
     const std::vector<int>& used = op->stages[0]->used_input_cols;
@@ -775,15 +782,11 @@ b200q_status b200q_op_push_ipc(b200q_op* op, const uint8_t* data, size_t len) {
 b200q_status b200q_op_push_device(b200q_op* op, struct ArrowDeviceArray* dbatch) {
   if (!op) return fail(B200Q_ERR_INVALID_ARG, "op is null");
   b200q_status st = guarded(op, [&] {
-    if (op->finished) throw ExecError(B200Q_ERR_STATE, "push after finish");
-    if (op->ipc) throw ExecError(B200Q_ERR_STATE, "an op whose leaf is an IpcReaderExecNode takes its input through b200q_op_push_ipc");
+    check_push_state(op);
     if (!dbatch) throw ExecError(B200Q_ERR_INVALID_ARG, "null batch");
     if (dbatch->device_type != ARROW_DEVICE_CUDA || dbatch->device_id != op->cx.device) throw ExecError(B200Q_ERR_INVALID_ARG, "push_device: batch is not on this op's CUDA device");
-    require_right_side(op);
-    B200Q_CUDA(cudaSetDevice(op->cx.device));
     ArrowArray* batch = &dbatch->array;
-    validate_host_batch(op, batch);
-    poll_pending(op, false);
+    begin_push(op, batch);
     if (op->staging_ready) staging_flush(op);
     if (dbatch->sync_event) B200Q_CUDA(cudaStreamWaitEvent(op->cx.stream, *(cudaEvent_t*)dbatch->sync_event, 0));
     op->cx.m.input_rows += batch->length; op->cx.m.input_batches++;
@@ -817,13 +820,9 @@ b200q_status b200q_op_finish(b200q_op* op) {
     if (op->finished) return;
     require_right_side(op);
     B200Q_CUDA(cudaSetDevice(op->cx.device));
-    {   // a ParquetScanExec leaf is the op's own source: read + decode the split now, one device batch per row group
-      const PlanNode* leaf = op->plan.get();
-      while (leaf->input) leaf = leaf->input.get();
-      if (leaf->kind == N_LEAF && leaf->leaf_kind == "ParquetScan") {
-        if (op->cx.m.input_batches) throw ExecError(B200Q_ERR_STATE, "an op whose leaf is a ParquetScanExecNode takes no pushed batches");
-        run_parquet_scan(op->cx, *leaf, [&](DevBatch& b) { run_stages(op, b, 0); });
-      }
+    if (op->leaf->leaf_kind == "ParquetScan") {   // the op's own source: read + decode the split now, one device batch per row group
+      if (op->cx.m.input_batches) throw ExecError(B200Q_ERR_STATE, "an op whose leaf is a ParquetScanExecNode takes no pushed batches");
+      run_parquet_scan(op->cx, *op->leaf, [&](DevBatch& b) { run_stages(op, b, 0); });
     }
     if (op->ipc) op->ipc->flush(op->cx, [&](DevBatch& b) { run_stages(op, b, 0); });
     if (op->staging_ready) staging_flush(op);
@@ -831,10 +830,7 @@ b200q_status b200q_op_finish(b200q_op* op) {
       std::vector<DevBatch> outs;
       op->cx.cur_stage = (int)i;
       op->stages[i]->finish(op->cx, outs);
-      for (auto& o : outs) {
-        if (i + 1 < op->stages.size()) run_stages(op, o, i + 1);
-        else { op->cx.m.output_rows += o.num_rows; op->out_queue.push_back(std::move(o)); }
-      }
+      route_outputs(op, i, outs);
     }
     B200Q_CUDA(cudaStreamSynchronize(op->cx.stream));
     poll_pending(op, true);
