@@ -378,7 +378,7 @@ static void poll_pending(b200q_op* op, bool wait) {
     cudaError_t q = wait ? cudaEventSynchronize(p.ev) : cudaEventQuery(p.ev);
     if (q == cudaSuccess || q != cudaErrorNotReady) {
       if (p.arr.release) p.arr.release(&p.arr);
-      cudaEventDestroy(p.ev);
+      event_put(op->cx.device, p.ev, false);
       op->pending.erase(op->pending.begin() + i);
     } else i++;
   }
@@ -719,7 +719,7 @@ b200q_status b200q_op_create(const uint8_t* plan, size_t plan_len, int32_t plan_
     }
     op->stream_ref = stream_ref_create(device);
     op->cx.stream = op->stream_ref->s;
-    B200Q_CUDA(cudaEventCreate(&op->cx.ev0)); B200Q_CUDA(cudaEventCreate(&op->cx.ev1));
+    op->cx.ev0 = event_get(device, true); op->cx.ev1 = event_get(device, true);
     build_pipeline(op);
     if (op->leaf->leaf_kind == "IpcReader") op->ipc = make_ipc_source(op->cx, op->in_schema, op->stages[0]->used_input_cols);
     if (input_schema) {
@@ -729,7 +729,7 @@ b200q_status b200q_op_create(const uint8_t* plan, size_t plan_len, int32_t plan_
           throw PlanError(B200Q_ERR_INVALID_ARG, "input_schema does not match the plan leaf: type of column " + std::to_string(i));
     }
   });
-  if (st != B200Q_OK) { if (op) { op->stages.clear(); delete op; } return st; }
+  if (st != B200Q_OK) { if (op) { op->stages.clear(); event_put(device, op->cx.ev0, true); event_put(device, op->cx.ev1, true); delete op; } return st; }
   *out = op;
   return B200Q_OK;
 }
@@ -757,7 +757,7 @@ b200q_status b200q_op_push(b200q_op* op, struct ArrowArray* batch) {
     DevBatch db = import_direct(op, batch, used);
     // the caller's buffers must outlive the async copies: release the batch when they have drained
     PendingRelease pr; pr.arr = *batch; batch->release = nullptr;
-    B200Q_CUDA(cudaEventCreateWithFlags(&pr.ev, cudaEventDisableTiming));
+    pr.ev = event_get(op->cx.device, false);
     B200Q_CUDA(cudaEventRecord(pr.ev, op->cx.stream));
     op->pending.push_back(pr);
     run_stages(op, db, 0);
@@ -803,7 +803,7 @@ b200q_status b200q_op_push_device(b200q_op* op, struct ArrowDeviceArray* dbatch)
     // queued BEFORE the stages run: if a stage throws, the array is still released (poll_pending) and the event destroyed;
     // in both cases the event is recorded behind the last kernel that reads the caller's buffers.
     PendingRelease pr; pr.arr = *batch;
-    B200Q_CUDA(cudaEventCreateWithFlags(&pr.ev, cudaEventDisableTiming));
+    pr.ev = event_get(op->cx.device, false);
     batch->release = nullptr;
     op->pending.push_back(pr);
     const cudaEvent_t ev = pr.ev;
@@ -903,10 +903,10 @@ void b200q_op_destroy(b200q_op* op) {
   op->ipc.reset();
   op->stages.clear();
   staging_free(op);
-  if (op->cx.ev0) cudaEventDestroy(op->cx.ev0);
-  if (op->cx.ev1) cudaEventDestroy(op->cx.ev1);
+  event_put(op->cx.device, op->cx.ev0, true);
+  event_put(op->cx.device, op->cx.ev1, true);
   if (op->cx.stream) cudaStreamSynchronize(op->cx.stream);
-  delete op;                     // the stream itself goes away with the last allocation that references it
+  delete op;                     // the stream returns to its pool with the last allocation that references it
 }
 
 b200q_status b200q_parquet_explain(const uint8_t* footer, size_t n, char* buf, size_t cap, size_t* needed) {

@@ -738,6 +738,14 @@ int launch_agg_emit(const AggLayout& lay, const AggTable& tab, const EmitTable& 
   return 1;
 }
 
+__global__ void copy_words_to_host_kernel(const unsigned long long* __restrict__ src, unsigned long long* __restrict__ dst, int n) {
+  if ((int)threadIdx.x < n) dst[threadIdx.x] = src[threadIdx.x];
+}
+int launch_copy_words_to_host(const unsigned long long* src, unsigned long long* pinned_dst, int n, cudaStream_t s) {
+  copy_words_to_host_kernel<<<1, 32, 0, s>>>(src, pinned_dst, n);
+  return 1;
+}
+
 __global__ void __launch_bounds__(256) pack_valid_kernel(const uint8_t* __restrict__ bytes, uint32_t* __restrict__ bits, long long n) {
   const long long nwords = (n + 31) / 32;
   const unsigned lane = threadIdx.x & 31;

@@ -141,6 +141,9 @@ int launch_agg_update_sets(const VmProgram* d_prog, const ColTable& cols, const 
                            const uint32_t* d_row_list, const AggSetDesc* d_sets, int nsets, uint64_t ord_base, cudaStream_t s);
 int launch_agg_rehash(const AggLayout& lay, const AggTable& old_tab, const AggTable& new_tab, cudaStream_t s);
 int launch_agg_emit(const AggLayout& lay, const AggTable& tab, const EmitTable& emit, unsigned long long* d_out_count, cudaStream_t s);
+// n (<= 32) words from device memory into pinned host memory (cudaMallocHost: addressable from the device at the same address), in
+// stream order and without a copy-engine operation: a D2H copy between two kernels of a stream leaves a bubble before the next one
+int launch_copy_words_to_host(const unsigned long long* src, unsigned long long* pinned_dst, int n, cudaStream_t s);
 int launch_pack_valid(const uint8_t* bytes, uint32_t* bits, int64_t n, cudaStream_t s);
 int launch_frozen_lengths(const FrozenTable& ft, int64_t n, int32_t* lengths, cudaStream_t s);
 int launch_exclusive_scan_i32(const int32_t* in, int32_t* out /* n+1 entries */, int64_t n, int32_t* d_block_sums, cudaStream_t s);

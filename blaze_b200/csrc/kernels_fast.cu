@@ -807,7 +807,15 @@ __global__ void __launch_bounds__(256) key_range_kernel(const DevCol col, int ph
     const long long a = __shfl_xor_sync(0xffffffffu, mn, d), b = __shfl_xor_sync(0xffffffffu, mx, d);
     mn = a < mn ? a : mn; mx = b > mx ? b : mx; cnt += __shfl_xor_sync(0xffffffffu, cnt, d);
   }
-  if ((threadIdx.x & 31) == 0) { atomicMin(out, mn); atomicMax(out + 1, mx); atomicAdd((unsigned long long*)out + 2, cnt); }
+  // one update of the three result words per CTA, not per warp: same-address atomics serialise in L2
+  __shared__ long long s_mn[8], s_mx[8]; __shared__ unsigned long long s_cnt[8];
+  const int w = threadIdx.x >> 5;
+  if ((threadIdx.x & 31) == 0) { s_mn[w] = mn; s_mx[w] = mx; s_cnt[w] = cnt; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int j = 1; j < (int)(blockDim.x >> 5); j++) { mn = s_mn[j] < mn ? s_mn[j] : mn; mx = s_mx[j] > mx ? s_mx[j] : mx; cnt += s_cnt[j]; }
+    atomicMin(out, mn); atomicMax(out + 1, mx); atomicAdd((unsigned long long*)out + 2, cnt);
+  }
 }
 int launch_key_skew_probe(const DevCol* key_cols, const uint8_t* phys, int nkeys, int64_t n, unsigned* d_hist, cudaStream_t s) {
   key_skew_hist_kernel<<<fast_grid((n + 2047) / 2048), 256, 0, s>>>(key_cols[0], key_cols[nkeys == 2 ? 1 : 0], phys[0], phys[nkeys == 2 ? 1 : 0], nkeys, n, d_hist);
@@ -833,26 +841,38 @@ __device__ __forceinline__ void dense_store(const EmitCol& c, unsigned long long
   }
 }
 __global__ void __launch_bounds__(256) agg_emit_dense_kernel(const FastSpec fs, const EmitTable emit, const DenseEmitMap map, unsigned long long* out_count) {
-  const unsigned lane = threadIdx.x & 31;
+  const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  __shared__ unsigned s_warp[8];
+  __shared__ unsigned long long s_base;
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   const uint64_t rounds = (fs.dense_cap + stride - 1) / stride;
+  const uint32_t r1 = (uint32_t)fs.dense_r1;                   // dense_cap <= 2^26 entries: key order indices fit 32 bits
   for (uint64_t it = 0; it < rounds; it++) {
-    const uint64_t i = it * stride + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;   // key order: (key0 - dense_base) * dense_r1 + (key1 - dense_base1)
-    const uint64_t pe = fs.nkeys == 2 && fs.dense_key0_minor ? dense_entry2(fs, i / fs.dense_r1, i % fs.dense_r1) : i;
+    const uint32_t i = (uint32_t)(it * stride + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x);   // key order: (key0 - dense_base) * dense_r1 + (key1 - dense_base1)
+    const uint32_t q = fs.nkeys == 2 ? i / r1 : i, r = fs.nkeys == 2 ? i - q * r1 : 0;
+    const uint64_t pe = fs.nkeys == 2 && fs.dense_key0_minor ? dense_entry2(fs, q, r) : i;
     const unsigned long long* e = fs.dense_tab + pe * fs.dense_stride;
     const bool occ = i < fs.dense_cap && e[fs.dense_presence_word] != 0;
     const unsigned m = __ballot_sync(0xffffffffu, occ);
-    if (!m) continue;
-    unsigned long long base = 0;
-    if (lane == 0) base = atomicAdd(out_count, (unsigned long long)__popc(m));
-    base = __shfl_sync(0xffffffffu, base, 0);
+    // one output reservation per CTA and round (a per-warp atomicAdd on the one counter serialises in L2); the warps of a CTA
+    // take consecutive runs, so the rows stay in key order within the CTA's round as they were within a warp
+    if (lane == 0) s_warp[warp] = __popc(m);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      unsigned tot = 0;
+      for (unsigned j = 0; j < nwarps; j++) { const unsigned c = s_warp[j]; s_warp[j] = tot; tot += c; }
+      s_base = tot ? atomicAdd(out_count, (unsigned long long)tot) : 0;
+    }
+    __syncthreads();
+    const unsigned long long base = s_base + s_warp[warp];
+    __syncthreads();                                            // s_warp / s_base are rewritten in the next round
     if (!occ) continue;
     const unsigned long long at = base + __popc(m & lanemask_lt());
     for (int c = 0; c < emit.ncols; c++) {
       const EmitCol ec = emit.col[c];
       if (ec.kind == EMIT_KEY) {
         const long long kv = fs.nkeys == 1 ? fs.dense_base + (long long)i
-                           : ec.key == 0 ? fs.dense_base + (long long)(i / fs.dense_r1) : fs.dense_base1 + (long long)(i % fs.dense_r1);
+                           : ec.key == 0 ? fs.dense_base + (long long)q : fs.dense_base1 + (long long)r;
         dense_store(ec, at, (uint64_t)kv, true);
       }
       else {

@@ -36,13 +36,17 @@ struct ExecError : std::runtime_error {
   } while (0)
 
 // The op's CUDA stream outlives the op while exported device arrays still reference allocations made on it
-// (their release frees stream-ordered memory): the stream is destroyed when the last reference goes away.
+// (their release frees stream-ordered memory): the stream returns to the device's pool when the last reference goes away.
 struct StreamRef {
   cudaStream_t s = nullptr; int device = 0;
   ~StreamRef();
 };
-std::shared_ptr<StreamRef> stream_ref_create(int device);
+std::shared_ptr<StreamRef> stream_ref_create(int device);      // a recycled stream of `device` when one is free
 std::shared_ptr<StreamRef> stream_ref_lookup(cudaStream_t s);
+// per-device pool of events (`timing`: created without cudaEventDisableTiming); get with `device` current.  An event may be
+// put back while a record of it is still pending: its next user records it again before waiting on it
+cudaEvent_t event_get(int device, bool timing);
+void event_put(int device, cudaEvent_t e, bool timing);
 
 // a device allocation (stream-ordered) or a borrowed device pointer kept alive by `owner`
 struct DevMem {

@@ -15,16 +15,44 @@ namespace b200q {
 // ---------------------------------------------------------------------------------------------------
 static std::mutex g_stream_mu;
 static std::unordered_map<cudaStream_t, std::weak_ptr<StreamRef>> g_streams;
+// Streams and events do not depend on the op: every op creating and destroying its own costs driver calls in every step, so
+// they are recycled per device.  A stream returns to its pool only when its StreamRef dies, that is when no op and no DevMem
+// (whose release frees stream-ordered memory on it) references it any more, and after its work has drained.
+struct CudaObjectPool { std::vector<cudaStream_t> streams; std::vector<cudaEvent_t> events[2]; };   // events[timing]
+static std::unordered_map<int, CudaObjectPool> g_pools;                                            // by device, under g_stream_mu
 
 StreamRef::~StreamRef() {
-  { std::lock_guard<std::mutex> l(g_stream_mu); g_streams.erase(s); }
-  if (s) { cudaSetDevice(device); cudaStreamSynchronize(s); cudaStreamDestroy(s); }
+  if (!s) return;
+  cudaSetDevice(device);
+  const bool drained = cudaStreamSynchronize(s) == cudaSuccess;
+  std::lock_guard<std::mutex> l(g_stream_mu);
+  g_streams.erase(s);
+  if (drained) g_pools[device].streams.push_back(s);
+  else cudaStreamDestroy(s);
 }
 std::shared_ptr<StreamRef> stream_ref_create(int device) {
   auto r = std::make_shared<StreamRef>(); r->device = device;
-  B200Q_CUDA(cudaStreamCreateWithFlags(&r->s, cudaStreamNonBlocking));
-  std::lock_guard<std::mutex> l(g_stream_mu); g_streams[r->s] = r;
+  std::lock_guard<std::mutex> l(g_stream_mu);
+  auto& free = g_pools[device].streams;
+  if (!free.empty()) { r->s = free.back(); free.pop_back(); }
+  else B200Q_CUDA(cudaStreamCreateWithFlags(&r->s, cudaStreamNonBlocking));
+  g_streams[r->s] = r;
   return r;
+}
+cudaEvent_t event_get(int device, bool timing) {
+  {
+    std::lock_guard<std::mutex> l(g_stream_mu);
+    auto& free = g_pools[device].events[timing];
+    if (!free.empty()) { cudaEvent_t e = free.back(); free.pop_back(); return e; }
+  }
+  cudaEvent_t e = nullptr;
+  B200Q_CUDA(timing ? cudaEventCreate(&e) : cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  return e;
+}
+void event_put(int device, cudaEvent_t e, bool timing) {
+  if (!e) return;
+  std::lock_guard<std::mutex> l(g_stream_mu);
+  g_pools[device].events[timing].push_back(e);
 }
 std::shared_ptr<StreamRef> stream_ref_lookup(cudaStream_t s) {
   std::lock_guard<std::mutex> l(g_stream_mu);
@@ -148,8 +176,8 @@ static DevMemP upload_program(const CompiledProgram& cp, cudaStream_t s, std::ve
     p.pool[b.pool_index] = (uint64_t)(uintptr_t)w->ptr;
     blooms.push_back(w);
   }
+  // `p` lives on this stack frame: a copy from pageable memory returns once its bytes are staged, so no wait is needed
   B200Q_CUDA(cudaMemcpyAsync(d->ptr, &p, sizeof(VmProgram), cudaMemcpyHostToDevice, s));
-  B200Q_CUDA(cudaStreamSynchronize(s));                 // `p` lives on this stack frame
   return d;
 }
 
@@ -824,7 +852,6 @@ class AggStage : public Stage {
     if (capacity_ >= (1ULL << 32)) throw PlanError(B200Q_ERR_UNSUPPORTED, "agg_initial_groups too large");
     alloc_table(cx, capacity_, keys_, accs_, counters_);
     if (lay_.nkeys == 0) seed_global_group(cx);
-    B200Q_CUDA(cudaStreamSynchronize(cx.stream));
     cx.m.table_capacity = (int64_t)capacity_;
   }
 
@@ -1066,14 +1093,21 @@ class AggStage : public Stage {
     for (int k = 0; k < nkeys; k++) cx.m.launches += launch_key_range(ct.col[key_col[k]], key_phys[k], sample, (long long*)d->ptr + 3 * k, cx.stream);
     DevMemP hist;
     if (probe_skew) {
-      hist = DevMem::alloc((65536 + 1) * 4, cx.stream, true);
+      hist = DevMem::alloc((65536 + 2) * 4, cx.stream, true);          // the maximum in word 65536, zero above it: one 64-bit word
       DevCol kc[2] = {ct.col[key_col[0]], ct.col[key_col[nkeys == 2 ? 1 : 0]]};
       cx.m.launches += launch_key_skew_probe(kc, key_phys, nkeys, sample, (unsigned*)hist->ptr, cx.stream);
     }
+    // the results come back through two pinned slots written in stream order (a D2H copy into pageable memory would wait
+    // for the stream by itself, once per copy): {min, max, non-null rows} of key 0 and the skew maximum, then those of key 1
     long long hr[6] = {0}; unsigned mx = 0;
-    B200Q_CUDA(cudaMemcpyAsync(hr, d->ptr, 48, cudaMemcpyDeviceToHost, cx.stream));
-    if (probe_skew) B200Q_CUDA(cudaMemcpyAsync(&mx, (unsigned*)hist->ptr + 65536, 4, cudaMemcpyDeviceToHost, cx.stream));
-    B200Q_CUDA(cudaStreamSynchronize(cx.stream));
+    {
+      struct Slots { unsigned long long* p[2]; ~Slots() { pinned_slots().put(p[0]); pinned_slots().put(p[1]); } } sl{{pinned_slots().get(), pinned_slots().get()}};
+      for (int k = 0; k < nkeys; k++) cx.m.launches += launch_copy_words_to_host((const unsigned long long*)d->ptr + 3 * k, sl.p[k], 3, cx.stream);
+      if (probe_skew) cx.m.launches += launch_copy_words_to_host((const unsigned long long*)hist->ptr + 32768, sl.p[0] + 3, 1, cx.stream);
+      B200Q_CUDA(cudaStreamSynchronize(cx.stream));
+      for (int k = 0; k < nkeys; k++) for (int j = 0; j < 3; j++) hr[3 * k + j] = (long long)sl.p[k][j];
+      if (probe_skew) mx = (unsigned)sl.p[0][3];
+    }
     long long nonnull = 0;
     for (int k = 0; k < nkeys; k++) {
       const long long* h = hr + 3 * k;                                     // {min, max, non-null rows}
@@ -1262,18 +1296,19 @@ class AggStage : public Stage {
     cx.m.num_groups = ngroups_;
   }
 
-  // The counters of a chunk (groups, deferred rows, error flags) are copied into a pinned snapshot right behind its kernel and read
+  // The counters of a chunk (groups, deferred rows, error flags) are written into a pinned snapshot right behind its kernel and read
   // while the NEXT chunk's kernel already runs: no host round trip between the launches of a batch.
   struct Snap { unsigned long long* h = nullptr; cudaEvent_t ready = nullptr, k0 = nullptr, k1 = nullptr; };
   Snap snap_[2];
+  int device_ = 0;
  public:
-  ~AggStage() override { for (auto& s : snap_) { if (s.h) pinned_slots().put(s.h); if (s.ready) cudaEventDestroy(s.ready); if (s.k0) cudaEventDestroy(s.k0); if (s.k1) cudaEventDestroy(s.k1); } }
-  void ensure_snaps() {
+  ~AggStage() override {
+    for (auto& s : snap_) { if (s.h) pinned_slots().put(s.h); event_put(device_, s.ready, false); event_put(device_, s.k0, true); event_put(device_, s.k1, true); }
+  }
+  void ensure_snaps(OpContext& cx) {
     if (snap_[0].h) return;
-    for (auto& s : snap_) {
-      s.h = pinned_slots().get();
-      B200Q_CUDA(cudaEventCreateWithFlags(&s.ready, cudaEventDisableTiming)); B200Q_CUDA(cudaEventCreate(&s.k0)); B200Q_CUDA(cudaEventCreate(&s.k1));
-    }
+    device_ = cx.device;
+    for (auto& s : snap_) { s.h = pinned_slots().get(); s.ready = event_get(device_, false); s.k0 = event_get(device_, true); s.k1 = event_get(device_, true); }
   }
   void account(OpContext& cx, const Snap& s, int64_t rows) {
     float ms = 0; B200Q_CUDA(cudaEventElapsedTime(&ms, s.k0, s.k1));
@@ -1305,7 +1340,7 @@ class AggStage : public Stage {
     static const bool dbg = getenv("B200Q_AGG_TIMING") != nullptr;
     auto hnow = [] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
     const double tA = hnow();
-    ensure_snaps();
+    ensure_snaps(cx);
     const double tB = hnow();
     const int64_t m_max = std::min(chunk, n);
     if (deferred_cap_ < 2 * m_max * nsets_) {                             // two chunks' worth: a chunk is launched before the counters of the one before it are back
@@ -1348,7 +1383,7 @@ class AggStage : public Stage {
       cx.m.launches += launch_update(cx, ct, table_view(0), begin, m, nullptr);
       B200Q_CUDA(cudaEventRecord(s.k1, cx.stream));
       B200Q_CUDA(cudaGetLastError());
-      B200Q_CUDA(cudaMemcpyAsync(s.h, counters_->ptr, 24, cudaMemcpyDeviceToHost, cx.stream));
+      cx.m.launches += launch_copy_words_to_host((const unsigned long long*)counters_->ptr, s.h, 3, cx.stream);
       B200Q_CUDA(cudaEventRecord(s.ready, cx.stream));
       const double ts = hnow(); t_launch += ts - tl;
       const bool slow = have_prev && settle((idx & 1) ^ 1, prev_begin, prev_m, true, begin, m);
@@ -1408,16 +1443,16 @@ class AggStage : public Stage {
   void finish(OpContext& cx, std::vector<DevBatch>& outs) override {
     // ONE host round trip for the group counts: the hash table's counters and the occupied entries of the dense / wide table land in one pinned slot
     const bool wide = wide_possible_ && ws_.dense_tab;
-    ensure_snaps();
+    ensure_snaps(cx);
     unsigned long long* hs = snap_[0].h;
     DevMemP dc;
     if (fs_.dense || wide) {
       dc = DevMem::alloc(8, cx.stream, true);
       if (wide) cx.m.launches += launch_tile_wide_normalise(ws_, cx.stream);
       cx.m.launches += fs_.dense ? launch_dense_count(fs_, (unsigned long long*)dc->ptr, cx.stream) : launch_tile_wide_count(ws_, (unsigned long long*)dc->ptr, cx.stream);
-      B200Q_CUDA(cudaMemcpyAsync(hs + 3, dc->ptr, 8, cudaMemcpyDeviceToHost, cx.stream));
+      cx.m.launches += launch_copy_words_to_host((const unsigned long long*)dc->ptr, hs + 3, 1, cx.stream);
     } else hs[3] = 0;
-    B200Q_CUDA(cudaMemcpyAsync(hs, counters_->ptr, 24, cudaMemcpyDeviceToHost, cx.stream));
+    cx.m.launches += launch_copy_words_to_host((const unsigned long long*)counters_->ptr, hs, 3, cx.stream);
     B200Q_CUDA(cudaStreamSynchronize(cx.stream));
     check_device_error_flags((int)hs[2]);
     ngroups_ = (int64_t)hs[0];
@@ -1438,7 +1473,8 @@ class AggStage : public Stage {
       ob.cols.push_back(c);
     }
     DevMemP out_count = DevMem::alloc(8, cx.stream, true);
-    cx.m.launches += launch_agg_emit(lay_, table_view(0), et, (unsigned long long*)out_count->ptr, cx.stream);
+    // the hashed slots hold ngroups_ groups (read above): with none, walking all of its slots would write nothing
+    if (ngroups_ > 0) cx.m.launches += launch_agg_emit(lay_, table_view(0), et, (unsigned long long*)out_count->ptr, cx.stream);
     if (fs_.dense) cx.m.launches += launch_agg_emit_dense(fs_, et, dmap_, (unsigned long long*)out_count->ptr, cx.stream);
     if (wide) cx.m.launches += launch_tile_wide_emit(ws_, lay_, et, (unsigned long long*)out_count->ptr, cx.stream);
     for (size_t i = 0; i < emit_.size(); i++) {
@@ -1470,7 +1506,6 @@ class AggStage : public Stage {
       ob.cols.resize(lay_.nkeys);
       ob.cols.push_back(bc);
     }
-    B200Q_CUDA(cudaStreamSynchronize(cx.stream));
     outs.push_back(std::move(ob));
   }
 };
